@@ -1,4 +1,4 @@
-# CUDA 12.9 + PyTorch image for B200 (sm_100a); the kernel library is compiled at image build time.
+# CUDA 12.9 + PyTorch image for H100 (sm_90a); the kernel library is compiled at image build time.
 FROM nvcr.io/nvidia/pytorch:25.06-py3
 WORKDIR /workspace/paddlefleetx_b200
 COPY . .

@@ -11,7 +11,7 @@ family-specific extras) and calls its family's ``run_benchmark.sh``.  This drive
    ``<LOG_DIR>/<model_name>_<device_num>_speed.json``.
 
 Synthetic data of the recipe's shape is used unless ``DATA_DIR`` points at a prepared corpus.  ``fp_item=fp16`` means "16-bit mixed precision",
-which on B200 is bf16 O2; ``fp32`` turns mixed precision off.  ``--dry-run`` prints the command without running it.
+which on H100 is bf16 O2; ``fp32`` turns mixed precision off.  ``--dry-run`` prints the command without running it.
 """
 import argparse
 import json

@@ -1,4 +1,4 @@
-"""Loader for the in-tree sm_100a kernel library.
+"""Loader for the in-tree sm_90a kernel library.
 
 Policy: on a machine with a CUDA device the native library is *required* — any op that receives a CUDA
 tensor raises if it cannot be loaded (no silent PyTorch fallback; set ``PFX_ALLOW_FALLBACK=1`` to opt in

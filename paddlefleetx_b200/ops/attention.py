@@ -2,8 +2,8 @@
 
 ``attention(q, k, v)`` takes ``[b, s, heads, d]`` tensors (views are fine: the slices of a packed QKV projection, sequence-major
 storage).  Path selection on CUDA / bf16:
-  * training and inference at head_dim 128 or 64: our tcgen05 / TMEM flash kernels — ``csrc/attention_fwd_sm100.cu`` and
-    ``csrc/attention_bwd_sm100.cu`` — with in-kernel causal masking and counter-hash dropout (the backward regenerates the mask; nothing is
+  * training and inference at head_dim 128 or 64: our wgmma flash kernels — ``csrc/attention_fwd_sm90.cu`` and
+    ``csrc/attention_bwd_sm90.cu`` — with in-kernel causal masking and counter-hash dropout (the backward regenerates the mask; nothing is
     stored).  ``flash_attention_packed`` is the same pair for the ``[b, s, heads, 3, d]`` output of a fused QKV projection: it reads q / k / v
     in place and writes ONE packed gradient, so no split / cat copies surround the kernels,
   * single-query decode steps over the static KV cache use ``csrc/attention_decode.cu`` (see models/.../gpt/model.py),

@@ -1,6 +1,6 @@
-"""In-tree AOT build of the sm_100a kernel library (``_pfx_native*.so``) and the C++ data helper.
+"""In-tree AOT build of the sm_90a kernel library (``_pfx_native*.so``) and the C++ data helper.
 
-``nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo`` for every ``.cu`` (they include no torch
+``nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo`` for every ``.cu`` (they include no torch
 headers, so each compiles in seconds), ``g++`` for the single pybind/torch binding file, one link.  The
 resulting ``.so`` lives next to this file so that it travels with the source tree to the GPU box; a content
 hash of the sources is stored beside it and the library is rebuilt only when the hash changes.
@@ -21,10 +21,10 @@ HERE = Path(__file__).resolve().parent
 CSRC = HERE / "csrc"
 BUILD_DIR = HERE / "csrc" / "build"
 MODULE_NAME = "_pfx_native"
-CUDA_SOURCES = ["gemm_sm100.cu", "norm_act.cu", "loss_optim.cu", "sampling_attn_misc.cu", "comm_p2p.cu",
-                "gemm_lowp_sm100.cu", "quant_kernels.cu", "moe_kernels.cu", "gemv_skinny.cu", "gemm_smallm_sm100.cu", "attention_decode.cu", "attention_fwd_sm100.cu", "comm_nvls.cu", "attention_bwd_sm100.cu", "evoformer_attn_sm100.cu", "embedding.cu", "probe_kernels.cu"]
+CUDA_SOURCES = ["gemm_sm90.cu", "norm_act.cu", "loss_optim.cu", "sampling_attn_misc.cu", "comm_p2p.cu",
+                "gemm_lowp_sm90.cu", "quant_kernels.cu", "moe_kernels.cu", "gemv_skinny.cu", "gemm_smallm_sm90.cu", "attention_decode.cu", "attention_fwd_sm90.cu", "comm_nvls.cu", "attention_bwd_sm90.cu", "evoformer_attn_sm90.cu", "embedding.cu"]
 CPP_SOURCES = ["bindings.cpp", "symm_vmm.cpp"]
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _ext_suffix() -> str:
@@ -90,7 +90,7 @@ def build(force: bool = False, verbose: bool = True) -> Path:
         list(pool.map(lambda j: _run(j[0], verbose), jobs))
 
     torch_lib = Path(torch.__file__).parent / "lib"
-    tmp_lib = BUILD_DIR / (lib_path().name + ".tmp")      # link beside, then rename: a concurrent reader (gpurun snapshot) never sees half a file
+    tmp_lib = BUILD_DIR / (lib_path().name + ".tmp")      # link beside, then rename: a concurrent reader never sees half a file
     link = ["g++", "-shared", "-o", str(tmp_lib), *[str(o) for _, o in jobs],
             f"-L{torch_lib}", f"-L{cuda_home}/lib64", "-lc10", "-lc10_cuda", "-ltorch_cpu", "-ltorch_cuda", "-ltorch",
             "-ltorch_python", "-lcudart", f"-Wl,-rpath,{torch_lib}", f"-Wl,-rpath,{cuda_home}/lib64"]

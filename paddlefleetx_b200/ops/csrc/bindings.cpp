@@ -1,4 +1,4 @@
-// pybind11 / torch glue for the sm_100a kernel library.  All kernels run on the current CUDA stream.
+// pybind11 / torch glue for the sm_90a kernel library.  All kernels run on the current CUDA stream.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -80,7 +80,7 @@ at::Tensor gemm(const at::Tensor& a, const at::Tensor& b, c10::optional<at::Tens
   g.out_mode = (int)out_mode; g.epilogue = (int)epilogue;
   g.ab_format = a.scalar_type() == at::kBFloat16 ? 1 : 0;
   g.num_sms = num_sms(); g.config = (int)config;
-  PFX_CUDA_CHECK(pfx::gemm_tcgen05(g, cur_stream()));
+  PFX_CUDA_CHECK(pfx::gemm_wgmma(g, cur_stream()));
   return d;
 }
 
@@ -97,7 +97,7 @@ std::vector<at::Tensor> gemm_bias_gelu_dual(const at::Tensor& x, const at::Tenso
   g.M = (int)x.size(0); g.N = (int)w.size(0); g.K = (int)x.size(1);
   g.lda = (int)x.stride(0); g.ldb = (int)w.stride(0); g.ldd = (int)z.stride(0);
   g.a_kmajor = true; g.b_kmajor = true; g.out_mode = 0; g.epilogue = pfx::EPI_BIAS_GELU_DUAL; g.ab_format = 1; g.num_sms = num_sms(); g.config = 0;
-  PFX_CUDA_CHECK(pfx::gemm_tcgen05(g, cur_stream()));
+  PFX_CUDA_CHECK(pfx::gemm_wgmma(g, cur_stream()));
   return {z, gl};
 }
 
@@ -114,7 +114,7 @@ at::Tensor gemm_dgelu(const at::Tensor& dy, const at::Tensor& w, const at::Tenso
   g.M = (int)dy.size(0); g.N = (int)w.size(1); g.K = (int)dy.size(1);
   g.lda = (int)dy.stride(0); g.ldb = (int)w.stride(0); g.ldd = (int)dz.stride(0);
   g.a_kmajor = true; g.b_kmajor = false; g.out_mode = 0; g.epilogue = pfx::EPI_DGELU; g.ab_format = 1; g.num_sms = num_sms(); g.config = 0;
-  PFX_CUDA_CHECK(pfx::gemm_tcgen05(g, cur_stream()));
+  PFX_CUDA_CHECK(pfx::gemm_wgmma(g, cur_stream()));
   return dz;
 }
 
@@ -136,7 +136,7 @@ void gemm_rs_scatter(const at::Tensor& a, const at::Tensor& b, const std::vector
   g.num_sms = num_sms(); g.config = config ? (int)config : 2;
   for (int i = 0; i < world; ++i) g.comm.peer_out[i] = reinterpret_cast<void*>((uintptr_t)peer_staging[i]);
   g.comm.rows_per_rank = (int)rows_per_rank; g.comm.my_rank = (int)my_rank; g.comm.world = world; g.comm.ag_world = 0;
-  PFX_CUDA_CHECK(pfx::gemm_tcgen05(g, cur_stream()));
+  PFX_CUDA_CHECK(pfx::gemm_wgmma(g, cur_stream()));
 }
 at::Tensor slot_reduce(const at::Tensor& staging, c10::optional<at::Tensor> bias, int64_t world) {
   PFX_CHECK_CUDA_CONTIG(staging);
@@ -174,7 +174,7 @@ at::Tensor gemm_ag(const at::Tensor& a_local, const at::Tensor& b, const at::Ten
   g.comm.a_local = a_local.data_ptr();
   g.comm.rows_per_rank = (int)rows; g.comm.chunk_rows = (int)chunk_rows; g.comm.my_rank = (int)my_rank; g.comm.world = world;
   g.comm.ag_world = world; g.comm.num_comm_ctas = (int)num_comm_ctas; g.comm.epoch = (uint32_t)epoch;
-  PFX_CUDA_CHECK(pfx::gemm_tcgen05(g, cur_stream()));
+  PFX_CUDA_CHECK(pfx::gemm_wgmma(g, cur_stream()));
   return d;
 }
 
@@ -208,7 +208,7 @@ at::Tensor gemm_lowp(const at::Tensor& a, const at::Tensor& b, c10::optional<at:
   g.M = (int)M; g.N = (int)N; g.K = (int)K; g.lda = (int)K; g.ldb = (int)K; g.ldd = (int)N;
   g.kind = a.scalar_type() == at::kChar ? 1 : 2;
   g.num_sms = num_sms(); g.config = (int)config;
-  PFX_CUDA_CHECK(pfx::gemm_lowp_tcgen05(g, cur_stream()));
+  PFX_CUDA_CHECK(pfx::gemm_lowp_wgmma(g, cur_stream()));
   return d;
 }
 
@@ -237,7 +237,7 @@ at::Tensor gemm_mxfp8(const at::Tensor& a, const at::Tensor& sfa, const at::Tens
   if (bias.has_value() && bias->defined()) { TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->numel() == N); g.bias = bias->data_ptr(); }
   g.M = (int)M; g.N = (int)N; g.K = (int)K; g.lda = (int)K; g.ldb = (int)K; g.ldd = (int)N;
   g.kind = 3; g.num_sms = num_sms(); g.config = 0;
-  PFX_CUDA_CHECK(pfx::gemm_lowp_tcgen05(g, cur_stream()));
+  PFX_CUDA_CHECK(pfx::gemm_lowp_wgmma(g, cur_stream()));
   return d;
 }
 
@@ -658,15 +658,6 @@ std::vector<at::Tensor> attention_fwd(const at::Tensor& q, const at::Tensor& k, 
   return {out, lse};
 }
 
-at::Tensor probe_tmem_a(const at::Tensor& a, const at::Tensor& b) {
-  PFX_CHECK_CUDA_CONTIG(a); PFX_CHECK_CUDA_CONTIG(b);
-  TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16 && a.size(0) == 128 && a.size(1) == 128 && b.size(0) == 64 && b.size(1) == 128,
-              "probe_tmem_a: a [128,128], b [64,128] bf16");
-  const c10::cuda::CUDAGuard guard(a.device());
-  auto d = at::empty({128, 64}, a.options().dtype(at::kFloat));
-  PFX_CUDA_CHECK(pfx::probe_tmem_a(a.data_ptr(), b.data_ptr(), d.data_ptr<float>(), cur_stream()));
-  return d;
-}
 
 // out[t] = w[ids[t] - vocab_start] (zero for foreign ids) (+ pos_w[pos[t]])
 at::Tensor embedding_fwd(const at::Tensor& ids, const at::Tensor& w, c10::optional<at::Tensor> pos, c10::optional<at::Tensor> pos_w, int64_t vocab_start) {
@@ -887,7 +878,7 @@ at::Tensor gemm_grouped(const at::Tensor& a, const at::Tensor& b, c10::optional<
   g.a_kmajor = true; g.b_kmajor = b_kmajor; g.out_mode = 0; g.epilogue = (int)epilogue; g.ab_format = 1; g.num_sms = num_sms(); g.config = 0;
   g.group.mode = 1; g.group.tile_group = tile_group.data_ptr<int>(); g.group.groups = (int)G; g.group.b_group_stride = (int)(b_kmajor ? N : K);
   g.group.row_align = (int)row_align;
-  PFX_CUDA_CHECK(pfx::gemm_tcgen05(g, cur_stream()));
+  PFX_CUDA_CHECK(pfx::gemm_wgmma(g, cur_stream()));
   return out;
 }
 
@@ -905,7 +896,7 @@ at::Tensor gemm_grouped_wgrad(const at::Tensor& dy, const at::Tensor& x, const a
   g.lda = (int)Mg; g.ldb = (int)N; g.ldd = (int)N;
   g.a_kmajor = false; g.b_kmajor = false; g.out_mode = 0; g.epilogue = pfx::EPI_NONE; g.ab_format = 1; g.num_sms = num_sms(); g.config = 0;
   g.group.mode = 2; g.group.seg = seg2.data_ptr<int>(); g.group.groups = (int)G; g.group.m_per_group = (int)Mg;
-  PFX_CUDA_CHECK(pfx::gemm_tcgen05(g, cur_stream()));
+  PFX_CUDA_CHECK(pfx::gemm_wgmma(g, cur_stream()));
   return out;
 }
 
@@ -931,7 +922,7 @@ void moe_combine(const std::vector<int64_t>& peer_src, const at::Tensor& slot_lo
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "paddlefleetx_b200 sm_100a kernel library";
+  m.doc() = "paddlefleetx_b200 sm_90a kernel library";
   m.def("gemm", &gemm, py::arg("a"), py::arg("b"), py::arg("bias") = py::none(), py::arg("out") = py::none(), py::arg("a_kmajor") = true,
         py::arg("b_kmajor") = true, py::arg("epilogue") = 0, py::arg("out_mode") = 0, py::arg("config") = 0);
   m.def("gemm_rs_scatter", &gemm_rs_scatter);
@@ -969,7 +960,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("p2p_reduce_scatter", &p2p_reduce_scatter);
   m.def("p2p_all_gather", &p2p_all_gather);
   m.def("attention_fwd", &attention_fwd);
-  m.def("probe_tmem_a", &probe_tmem_a);
   m.def("moe_tile_table", &moe_tile_table);
   m.def("quantize_mxfp8", &quantize_mxfp8);
   m.def("gemm_mxfp8", &gemm_mxfp8, py::arg("a"), py::arg("sfa"), py::arg("b"), py::arg("sfb"), py::arg("bias") = py::none());

@@ -11,10 +11,10 @@
 //   * all-gather       same store path for plain shards (ZeRO-3 parameter gather, tests).
 //   * barrier          one multimem.red (+1 on every rank's flag word) + a local acquire spin.
 //
-// Every kernel is 256 threads, <= 72 registers and ZERO shared memory (static included): a CTA fits next to a persistent tcgen05 GEMM
-// CTA (256 threads x <= 160 registers; the GEMM leaves 12 KB of the SM's shared memory free for exactly this) on the same SM, so communication CTAs neither wait for a GEMM wave to
-// drain nor park GEMM clusters behind themselves — which is what happens with NCCL's kernels (their shared-memory
-// footprint does not fit beside the GEMM) and what round 1 measured as a fixed ~12 ms / step scaling loss.
+// Every kernel is 256 threads, <= 72 registers and ZERO shared memory (static included), so that a CTA takes little of an SM.  It does
+// NOT fit beside a persistent wgmma GEMM CTA: that one holds 288 threads x 168 registers (about 50 K of the SM's 64 K registers), and 256 x 72
+// more do not fit.  Communication CTAs therefore get SMs when a GEMM CTA retires, not a place inside a busy SM; the overlap of these kernels
+// with the GEMMs has not been run on H100.
 //
 // Reference call sites: sharding reduce / broadcast overlap knobs, eager_engine.py:293-307 (NCCL launches in Paddle).
 #include "pfx_common.cuh"

@@ -160,8 +160,7 @@ cudaError_t launch_rows(const T* x, const T* w, const T* bias, T* y, int N, int 
   const long groups = (N + cols - 1) / cols;
   int split = 1;
   if (kRows == 1) {
-    // measured sweep on B200 (profiles/selftest_r1_call18.jsonl): 4 rows per warp with the block's warps split 2-way over K is best
-    // or within 2 % of best for every GPT-6.7B decode shape; very long K (FFN2) prefers 8 slices
+    // 4 rows per warp with the block's warps split 2-way over K; very long K (FFN2) gets 8 slices
     split = K >= 16384 ? 8 : (K >= 2048 ? 2 : 1);
   } else {
     while (split < 8 && groups * split < target && K / (split * 2) >= 1024) split *= 2;

@@ -1,4 +1,4 @@
-// Flash-attention kernels (attention_fwd_sm100.cu, attention_bwd_sm100.cu): host interface and the shared dropout generator.
+// Flash-attention kernels (attention_fwd_sm90.cu, attention_bwd_sm90.cu): host interface and the shared dropout generator.
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

@@ -1,4 +1,4 @@
-// Host-side C++ interface of the tcgen05 GEMM family (no torch headers: keeps .cu compiles fast).
+// Host-side C++ interface of the wgmma GEMM family (no torch headers: keeps .cu compiles fast).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -62,7 +62,7 @@ struct GemmArgs {
   GemmGroup group;   // mode 0 = plain GEMM
 };
 
-cudaError_t gemm_tcgen05(const GemmArgs& args, cudaStream_t stream);
+cudaError_t gemm_wgmma(const GemmArgs& args, cudaStream_t stream);
 
 // 8-bit GEMM: D(bf16)[M,N] = (A_q[M,K] * B_q[N,K]^T) * row_scale[M] * col_scale[N] (+ bias[N]); both operands K-major.
 struct LowpGemmArgs {
@@ -76,7 +76,7 @@ struct LowpGemmArgs {
   const void* sfa = nullptr;   // kind 3: E8M0 scale bytes of A / B, one 512-byte atom per (128 rows, 128 K): [row_blocks, K / 128, 512]
   const void* sfb = nullptr;
 };
-cudaError_t gemm_lowp_tcgen05(const LowpGemmArgs& args, cudaStream_t stream);
+cudaError_t gemm_lowp_wgmma(const LowpGemmArgs& args, cudaStream_t stream);
 
 // hit / miss counters of the tensor-map descriptor cache (diagnostics)
 void tmap_cache_stats(uint64_t* hits, uint64_t* misses);

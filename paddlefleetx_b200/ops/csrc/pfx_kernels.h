@@ -62,11 +62,11 @@ void gemv_set_tuning(int cols, int split);
 cudaError_t gemv_w8a8(const void* x, const void* w, const float* xs, const float* ws, const void* bias, void* y, int M, int N, int K, int num_sms,
                       cudaStream_t st);
 
-// gemm_smallm_sm100.cu — swap-AB tcgen05 GEMM, split-K over a cluster with DSMEM reduction (1 <= M <= 128, bf16)
+// gemm_smallm_sm90.cu — swap-AB wgmma GEMM, split-K over a cluster with DSMEM reduction (1 <= M <= 128, bf16)
 cudaError_t gemm_smallm(const void* x, const void* w, const void* bias, void* y, int M, int N, int K, int dtype, int split, int num_sms,
                         cudaStream_t st);
 
-// attention_fwd_sm100.cu — flash-style attention forward (tcgen05 / TMEM / TMA), [B,S,H,D] bf16, D in {64,128}
+// attention_fwd_sm90.cu — flash-style attention forward (wgmma / TMA), [B,S,H,D] bf16, D in {64,128}
 cudaError_t attention_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Sq, int Sk, int H, int D, float scale,
                           bool causal, cudaStream_t st);
 
@@ -74,8 +74,6 @@ cudaError_t attention_fwd(const void* q, const void* k, const void* v, void* out
 cudaError_t attention_decode(const void* q, void* k, void* v, const void* mask, void* out, int B, int H, int D, int L, int Lmax,
                              float scale, int dtype, cudaStream_t st, const int64_t* write_idx = nullptr);
 
-// probe_kernels.cu — hardware semantics probes (run by tools/gpu_selftest.py)
-cudaError_t probe_tmem_a(const void* a, const void* b, float* d, cudaStream_t st);
 
 // embedding.cu — fused word (+ position) look-up; deterministic sorted scatter-add gradient (workspace: next_pow2(tokens) 64-bit keys)
 cudaError_t embedding_fwd(const int64_t* ids, const void* w, const int64_t* pos, const void* pw, void* out, int64_t tokens, int hidden,

@@ -1,5 +1,5 @@
-// Thin inline-PTX layer for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM),
-// cluster helpers.  Everything the kernels in this directory need and nothing else — no CUTLASS.
+// Thin inline-PTX layer for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), cluster helpers; the wgmma wrappers live in
+// pfx_wgmma.cuh.  Everything the kernels in this directory need and nothing else — no CUTLASS.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -7,6 +7,8 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
+
+#include "pfx_wgmma.cuh"
 
 #ifndef PFX_HANG_GUARD
 #define PFX_HANG_GUARD 1  // trap instead of spinning forever on a lost mbarrier arrival
@@ -90,10 +92,8 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if ((++polls & 0xFFFu) == 0u) {
       const long long now = clock64();
       if (t0 == 0) t0 = now;
-      else if (now - t0 > 4000000000ll) {  // ~2 s at B200 clocks: a lost arrival, not a slow producer
-        printf("pfx: mbarrier timeout block=%d thread=%d bar=%u parity=%u\n", (int)blockIdx.x, (int)threadIdx.x, bar, parity);
-        __trap();
-      }
+      else if (now - t0 > 4000000000ll) __trap();  // ~2 s at H100 clocks: a lost arrival, not a slow producer.  No printf here: a function call in
+                                                   // this inlined wait makes ptxas serialise every wgmma of the calling kernel (C7510)
     }
   }
 #else
@@ -110,14 +110,6 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint32_t bar, 
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-// 2-CTA variant: data lands in the issuing CTA's smem, bytes are credited to the *leader* CTA's
-// barrier (peer bit 24 of the shared::cluster address cleared).
-__device__ __forceinline__ void tma_load_2d_2sm(const CUtensorMap* m, uint32_t bar, uint32_t dst, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & 0xFEFFFFFFu), "r"(c0), "r"(c1)
       : "memory");
 }
 // 3-D tile load (attention: [columns, sequence, batch] views with arbitrary sequence / batch strides)
@@ -152,169 +144,6 @@ template <int N>
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 template <int N>
 __device__ __forceinline__ void tma_store_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
-
-// ------------------------------------------------------------------ tcgen05 / TMEM
-template <int kCtaGroup>
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  if constexpr (kCtaGroup == 1)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  else
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-}
-template <int kCtaGroup>
-__device__ __forceinline__ void tmem_relinquish() {
-  if constexpr (kCtaGroup == 1) asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  else asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int kCtaGroup>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  if constexpr (kCtaGroup == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  else asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers bf16/fp16 inputs with fp32 accumulate.
-template <int kCtaGroup>
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (kCtaGroup == 1)
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-  else
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n}\n"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// int8 x int8 -> int32
-template <int kCtaGroup>
-__device__ __forceinline__ void umma_i8(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (kCtaGroup == 1)
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n}\n"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-  else
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::i8 [%0], %1, %2, %3, p;\n}\n"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// fp8 (e4m3/e5m2) -> fp32
-template <int kCtaGroup>
-__device__ __forceinline__ void umma_f8(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (kCtaGroup == 1)
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n}\n"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-  else
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], %1, %2, %3, p;\n}\n"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-
-// Block-scaled fp8 (MX: one E8M0 scale per 32 K-elements per row), cta_group::1.  Scale factors live in tensor memory: tsfa / tsfb are
-// the TMEM column addresses of A's and B's scale words (lane = row % 32, replicated in the four lane quarters; column = row / 32; the
-// byte inside the 32-bit word = the idesc's a_sf_id / b_sf_id, i.e. which of the four 32-element K blocks of a 128-wide stage).
-__device__ __forceinline__ void umma_mxf8(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t tsfa, uint32_t tsfb,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(tsfa), "r"(tsfb) : "memory");
-}
-// Instruction descriptor of kind::mxf8f6f4.block_scale (e4m3 x e4m3, E8M0 scales, both operands K-major):
-//   b_sf_id [4,6)  a_format [7,10)  b_format [10,13)  n_dim [17,23) = N >> 3  scale_format bit 23 (1 = E8M0)  m_dim [24,29) = M >> 4  a_sf_id [29,31)
-__host__ __device__ constexpr uint32_t umma_idesc_mxf8(uint32_t M, uint32_t N, uint32_t a_sf_id, uint32_t b_sf_id) {
-  return (b_sf_id << 4) | ((N >> 3) << 17) | (1u << 23) | ((M >> 4) << 24) | (a_sf_id << 29);
-}
-// shared memory -> tensor memory copy of one scale-factor atom: 32 rows x 128 bits, broadcast to the four 32-lane quarters
-__device__ __forceinline__ void tmem_cp_32x128b_warpx4(uint32_t dst_tmem, uint64_t smem_desc) {
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(dst_tmem), "l"(smem_desc) : "memory");
-}
-// descriptor of an unswizzled K-major region: 8-row groups `sbo_bytes` apart (the scale-factor atoms: 8 x 16 B = 128)
-__device__ __forceinline__ uint64_t umma_desc_noswizzle(uint32_t smem_addr, uint32_t sbo_bytes) {
-  return uint64_t((smem_addr >> 4) & 0x3FFF) | (uint64_t((sbo_bytes >> 4) & 0x3FFF) << 32) | (uint64_t(1) << 46);
-}
-
-// commit: arrive on `bar` once every MMA issued so far by this thread has retired.
-template <int kCtaGroup>
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  if constexpr (kCtaGroup == 1)
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-  else  // arrive on the same barrier offset in both CTAs of the pair
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(bar), "h"((uint16_t)0x3) : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (one row per thread).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM: this warp's 32 lanes x 32 consecutive fp32 columns (one row per thread)
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-        "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]),
-        "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-// registers -> TMEM: 32 lanes x 16 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-        "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]: the A operand is read from tensor memory (lane = row, one 32-bit column = two consecutive K
-// elements; layout verified on the part by probe_kernels.cu)
-__device__ __forceinline__ void umma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n}\n"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ------------------------------------------------------------------ UMMA descriptors
-// Shared-memory matrix descriptor (SM100 "version 1"), 128-byte swizzle.
-//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version = 1      bits [61,64) layout (2 = SW128)
-__host__ __device__ constexpr uint64_t umma_desc_hi_lo(uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return (uint64_t((lbo_bytes >> 4) & 0x3FFF) << 16) | (uint64_t((sbo_bytes >> 4) & 0x3FFF) << 32) |
-         (uint64_t(1) << 46) | (uint64_t(2) << 61);
-}
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint64_t hi_lo_template) {
-  return hi_lo_template | uint64_t((smem_addr >> 4) & 0x3FFF);
-}
-
-// Instruction descriptor for kind::f16 / kind::i8 / kind::f8f6f4 (dense, no negate, no saturate).
-//   c_format [4,6): 0=f16 1=f32 2=s32 ; a_format [7,10), b_format [10,13) ; a_major bit15, b_major bit16 (1 = MN-major)
-//   n_dim [17,23) = N>>3 ; m_dim [24,29) = M>>4
-__host__ __device__ constexpr uint32_t umma_idesc(uint32_t c_fmt, uint32_t a_fmt, uint32_t b_fmt, bool a_mn_major, bool b_mn_major,
-                                                  uint32_t M, uint32_t N) {
-  return (c_fmt << 4) | (a_fmt << 7) | (b_fmt << 10) | (uint32_t(a_mn_major) << 15) | (uint32_t(b_mn_major) << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
-}
 
 // ------------------------------------------------------------------ misc math
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {

@@ -33,8 +33,8 @@ void unmap(int64_t ptr);
 }  // namespace vmm
 
 // ---- comm_nvls.cu: collectives over multicast (NVLS) and unicast peer addresses; dtype codes 0 = fp16, 1 = bf16, 3 = fp32.
-// All kernels use <= 64 registers / thread, 256 threads and no shared memory beyond a few words so that their CTAs
-// co-reside with a persistent tcgen05 GEMM CTA on the same SM instead of waiting for it (or making it wait).
+// All kernels use <= 64 registers / thread, 256 threads and no shared memory beyond a few words to stay small; beside
+// the wgmma GEMM CTA (288 threads x 168 registers) they do not fit on the same SM any more (see comm_nvls.cu).
 
 // Barrier over the group on the stream: one multimem.red (+1 on every rank's flag) and a local spin until `target` arrivals.
 cudaError_t nvls_barrier(uint32_t* mc_flag, uint32_t* local_flag, uint32_t target, cudaStream_t st);

@@ -1,4 +1,4 @@
-// Dynamic quantisation kernels feeding the 8-bit tcgen05 GEMMs: per-row (per-token) abs-max scaling to int8 or fp8
+// Dynamic quantisation kernels feeding the 8-bit wgmma GEMMs: per-row (per-token) abs-max scaling to int8 or fp8
 // e4m3 in one pass (row kept in registers), optional SmoothQuant per-channel divisor folded in.
 #include <cuda_fp8.h>
 
@@ -68,7 +68,7 @@ cudaError_t quantize_rows(const void* x, const float* smooth, void* q, float* sc
 // ---------------------------------------------------------------------------------------------------------------- MX fp8
 // x [rows, K] (bf16 / fp16) -> q e4m3 [rows, K] + E8M0 block scales, one per 32 consecutive K-elements of a row, chosen as the
 // smallest power of two that brings the block's maximum inside the e4m3 range (448).  The scale bytes are written directly in the
-// order the GEMM's smem -> TMEM copy consumes (gemm_lowp_sm100.cu): atom (row / 128, k / 128) of 512 bytes, byte
+// order the MX GEMM reads (gemm_lowp_sm90.cu): atom (row / 128, k / 128) of 512 bytes, byte
 // (row % 32) * 16 + ((row % 128) / 32) * 4 + (k / 32) % 4.  One thread per 32-element block: 64 B in, 32 B + 1 B out.
 namespace {
 template <typename T>

@@ -2,8 +2,8 @@
 
     out[g, q, h, :] = softmax_k(scale * q.k + mask_bias[g, k] + pair_bias[g // groups_per_pair, h, q, k]) @ v * sigmoid(gate)
 
-Forward: one tcgen05 kernel (``csrc/evoformer_attn_sm100.cu``) — logits, both biases, softmax, P V and the gate never leave the chip; only the
-output and the row-wise log-sum-exp are written.  Backward: a second tcgen05 kernel recomputes the probabilities per tile from (q, k, biases,
+Forward: one wgmma kernel (``csrc/evoformer_attn_sm90.cu``) — logits, both biases, softmax, P V and the gate never leave the chip; only the
+output and the row-wise log-sum-exp are written.  Backward: a second wgmma kernel recomputes the probabilities per tile from (q, k, biases,
 lse) and produces dq / dk / dv / dgate and the pair-bias gradient (fp32 reductions over the groups that share a bias); nothing of size
 [g, h, q, k] is ever stored (the reference keeps logits, probabilities and the gated average of all 48 blocks x 6 attentions alive).
 ``PFX_EVO_BWD=torch`` selects the older chunked recomputation with library matmuls (also used when the mask bias needs a gradient).
@@ -20,7 +20,7 @@ import torch
 from . import _native
 
 _CHUNK_ELEMS = 1 << 27          # probabilities materialised per backward chunk (fp32 elements)
-_BWD = os.environ.get("PFX_EVO_BWD", "native")      # "native" = tcgen05 backward kernel, "torch" = chunked recomputation with library matmuls
+_BWD = os.environ.get("PFX_EVO_BWD", "native")      # "native" = wgmma backward kernel, "torch" = chunked recomputation with library matmuls
 
 
 def reference(q, k, v, mask_bias, pair_bias, gate, groups_per_pair: int, scale: float):
@@ -73,7 +73,7 @@ class _EvoAttnFn(torch.autograd.Function):
         dout = dout.contiguous()
         need_mb = has_mb and ctx.needs_input_grad[3]
         if _BWD == "native" and q.is_cuda and len(ctx.saved_tensors) == 8 and not need_mb:
-            # one tcgen05 kernel (csrc/evoformer_attn_sm100.cu): five products per (group, head, key tile), pair-bias gradient by fp32 reds
+            # one wgmma kernel (csrc/evoformer_attn_sm90.cu): five products per (group, head, key tile), pair-bias gradient by fp32 reds
             lib = _native.require()
             out = ctx.saved_tensors[7]
             need_pb = has_pb and ctx.needs_input_grad[4]

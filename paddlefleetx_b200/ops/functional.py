@@ -1,6 +1,6 @@
 """Functional op layer: every hot op of the model zoo goes through one of these.
 
-On CUDA (bf16/fp16) the call lands in the hand-written sm_100a kernels of ``csrc/`` through an
+On CUDA (bf16/fp16) the call lands in the hand-written sm_90a kernels of ``csrc/`` through an
 ``autograd.Function``; on CPU (and for fp32 debugging runs) the plain PyTorch expression next to it is used —
 that expression is also the numerical reference in ``tests/``.  There is no runtime backend dispatch beyond
 this device check: a CUDA tensor with a missing native library raises.
@@ -22,7 +22,7 @@ from ..parallel.rng import get_rng_state_tracker
 
 _LOWP = (torch.bfloat16, torch.float16)
 _SMALLM = os.environ.get("PFX_SMALLM_GEMM", "1") == "1"
-_GEMV_MAX_ROWS = 2 if _SMALLM else 8       # measured on B200: the swap-AB tcgen05 kernel wins from 3 rows up (profiles/README.md)
+_GEMV_MAX_ROWS = 2 if _SMALLM else 8       # the swap-AB wgmma kernel serves 3 rows and up
 
 # launch accounting for bench.py ("gpu_launches": kernels of OURS inside the timed region)
 _launch_count = 0
@@ -138,7 +138,7 @@ def fused_ffn(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2: torch.Ten
 
 
 class _LinearFn(torch.autograd.Function):
-    """y = x W^T (+ b).  fwd: TN tcgen05 GEMM with bias epilogue; dgrad: NN GEMM (B MN-major, no transpose
+    """y = x W^T (+ b).  fwd: TN wgmma GEMM with bias epilogue; dgrad: NN GEMM (B MN-major, no transpose
     copy); wgrad: TN GEMM with both operands MN-major, optionally accumulating straight into an fp32
     ``main_grad`` buffer (reference amp.py:44-63 does that with a separate elementwise hook)."""
 
@@ -186,7 +186,7 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
     if (_SMALLM and x.is_cuda and x.dtype == torch.bfloat16 and weight.dtype == torch.bfloat16 and weight.is_contiguous()
             and x.numel() // x.shape[-1] <= 128 and x.shape[-1] % 8 == 0 and weight.shape[0] % 8 == 0
             and not (torch.is_grad_enabled() and (x.requires_grad or weight.requires_grad)) and _native.available()):
-        # prefill / batched decode: swap-AB tcgen05 GEMM, split-K over a cluster (csrc/gemm_smallm_sm100.cu)
+        # prefill / batched decode: swap-AB wgmma GEMM, split-K over a cluster (csrc/gemm_smallm_sm90.cu)
         _count()
         y = _native.require().gemm_smallm(x.reshape(-1, x.shape[-1]).contiguous(), weight, bias, 0)
         return y.view(*x.shape[:-1], weight.shape[0])

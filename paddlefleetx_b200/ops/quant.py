@@ -1,4 +1,4 @@
-"""Quantised linear layers on the 8-bit tcgen05 GEMMs.
+"""Quantised linear layers on the 8-bit wgmma GEMMs.
 
 ``Int8Linear``  — W8A8 inference layer: int8 weights with per-output-channel scales (from QAT abs-max statistics or from
                   post-training SmoothQuant), activations quantised per token on the fly (``quantize_rows`` kernel, optional

@@ -124,13 +124,12 @@ class FusedAdamW:
         # runs underneath the compute-bound GEMMs of the next forward pass instead of in front of it.  Needs direct gradient writes (no
         # memset of the gradient buffer between step and backward) and the device-resident native update.
         self.step_overlap = (bool(step_overlap) or self.use_p2p) and named[0][1].is_cuda and not self.offload
-        # measured on 2 x B200 (6.7B step): 16 / 64 / 296 reduce-scatter CTAs -> 368.9 / 321.5 / 315.6 ms per step: the kernels co-reside with the
-        # GEMMs, and the shorter they run the less GEMM time they perturb
-        self._rs_ctas = int(_os.environ.get("PFX_RS_CTAS", "296"))
-        # grid cap of the side-stream AdamW (0 = 8 CTAs per SM).  At full width the update takes the whole memory system and the forward GEMMs
-        # beside it run 2-3x slower; 2 CTAs per SM measured best on one B200 (6.7B step: 339.9 ms uncapped / 336.5 @148 / 328.9 @296, same box)
-        self._adamw_ctas = int(_os.environ.get("PFX_ADAMW_CTAS", "296"))
-        self._bcast_ctas = int(_os.environ.get("PFX_BCAST_CTAS", "296"))
+        # the side-stream kernels co-reside with the GEMMs, and the shorter they run the less GEMM time they perturb: 2 CTAs per SM each
+        # (at full width the AdamW update takes the whole memory system and the forward GEMMs beside it slow down)
+        two_per_sm = str(2 * torch.cuda.get_device_properties(named[0][1].device).multi_processor_count) if named[0][1].is_cuda else "264"
+        self._rs_ctas = int(_os.environ.get("PFX_RS_CTAS", two_per_sm))
+        self._adamw_ctas = int(_os.environ.get("PFX_ADAMW_CTAS", two_per_sm))      # 0 = 8 CTAs per SM
+        self._bcast_ctas = int(_os.environ.get("PFX_BCAST_CTAS", two_per_sm))
 
         # ---- bucket assignment (reverse registration order: last layers finish backward first)
         bucket_bytes = bucket_mb * 1024 * 1024 if (self.replicas > 1 or self.step_overlap) else (1 << 62)
@@ -195,7 +194,7 @@ class FusedAdamW:
             if self.offload:
                 # reference ``sharding_offload`` (group_sharded stage 2 + CPU offload, eager_engine.py:295-307): fp32 master weights and both
                 # moments live in (pinned) host memory, the update runs on the host and only the low-precision weights return to the device.
-                # With 180 GB per GPU this is a capacity escape hatch, not a performance path.
+                # With 80 GB per GPU this is a capacity escape hatch, not a performance path.
                 pin = dev.type == "cuda"
                 g.meta["has_master"] = True
                 for k2 in ("master", "m", "v"):

@@ -9,7 +9,7 @@ step's bytes, which look like perfectly good numbers.  This mode makes those bug
   ``check_finite`` names the buffer, the rank and the first bad element;
 * **epoch-skew check** — every rank must have issued the same number of barriers on every channel; ``barrier_skew_check`` compares the
   host-side counters across the group (a mismatch means some rank will satisfy another rank's *next* barrier with a stale arrival);
-* race detection itself is ``compute-sanitizer --tool racecheck`` on the single-GPU kernels: ``tools/gpu_sanitize.sh``.
+* race detection itself is ``compute-sanitizer --tool racecheck`` around ``tools/gpu_selftest.py <check>``.
 
 Everything here costs host synchronisation and memory traffic; nothing runs unless the environment variable is set.
 """

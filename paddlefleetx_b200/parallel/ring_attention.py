@@ -12,7 +12,7 @@ first attends to one, and the step time is the maximum:
   * block from a rank ``j < r``: all local queries see its FIRST chunk, none see its second  ->  ``q x k[:half]``, unmasked;
   * block from a rank ``j > r``: only the local SECOND chunk sees it, and sees all of it     ->  ``q[half:] x k``, unmasked.
 
-Every block is one call of the flash kernels (``csrc/attention_fwd_sm100.cu`` returns the row log-sum-exp, ``attention_bwd_sm100.cu`` takes
+Every block is one call of the flash kernels (``csrc/attention_fwd_sm90.cu`` returns the row log-sum-exp, ``attention_bwd_sm90.cu`` takes
 the FINAL log-sum-exp and output, which is all a block's backward needs: ``P = exp(S - lse)``, ``delta = rowsum(dO o O)``); partial outputs
 are merged with the usual online-softmax rescaling in fp32.  The transfer of the next block is posted before the current block is computed
 (``batch_isend_irecv``: NCCL p2p on its own internal stream on CUDA, gloo on CPU), so the exchange hides behind the attention math.  In the

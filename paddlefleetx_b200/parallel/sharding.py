@@ -284,7 +284,7 @@ class GroupShardedStage3(nn.Module):
                     sm, ch = self._symm, self._chan()
                     sm.barrier(channel=ch)
                     self._lib.symm_reduce_scatter(sm.mc_ptr(gf) if self.world >= 4 else 0, sm.peer_ptrs(gf), self.rank * s, piece, self.rank,
-                                                  {torch.float16: 0, torch.bfloat16: 1, torch.float32: 3}[gf.dtype], 1.0, False, None, 148)
+                                                  {torch.float16: 0, torch.bfloat16: 1, torch.float32: 3}[gf.dtype], 1.0, False, None, torch.cuda.get_device_properties(gf.device).multi_processor_count)
                     sm.barrier(channel=ch)
                     self._pool_give(gf)
                 elif gf.is_cuda:

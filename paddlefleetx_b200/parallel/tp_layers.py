@@ -11,7 +11,7 @@ gpt/dygraph/hybrid_model.py:139-196,589-605,699-704,951-952) and from its in-tre
     VocabParallelEmbedding     vocab-sharded lookup + all-reduce
     ParallelCrossEntropy       vocab-parallel softmax-CE
 
-Weights are stored ``[out, in]`` (torch convention, K-major for the tcgen05 GEMM).  ``mp_group=None`` or a
+Weights are stored ``[out, in]`` (torch convention, K-major for the wgmma GEMM).  ``mp_group=None`` or a
 size-1 group degenerates every layer to its plain single-GPU form, so the same model code serves 1..N GPUs.
 With ``Fused.tp_comm`` enabled on NVSwitch boxes the SP linears run the fused GEMM+collective kernels of
 ``parallel/fused_tp.py`` instead of NCCL + GEMM.
@@ -29,7 +29,7 @@ from . import comm_ops as C
 # process-wide defaults taken from the YAML ``Fused`` section (``configure`` is called by the task modules before the model is
 # built): ``tp_comm`` = fused all-gather->GEMM / GEMM->reduce-scatter kernels in the SP linears, ``fp8_tp_gemm`` = forward GEMMs of
 # the tensor-parallel linears in fp8-e4m3, backward in bf16; ``fp8_recipe`` = "mx" (default: OCP MX block scaling, one E8M0 scale per 32
-# K-elements applied by the tensor core, tcgen05 kind::mxf8f6f4.block_scale) or "rowwise" (per-token x per-channel fp32 scales in the epilogue)
+# K-elements folded in by the GEMM's consumer threads) or "rowwise" (per-token x per-channel fp32 scales in the epilogue)
 _OPTIONS = {"tp_comm": False, "fp8_tp_gemm": False, "fp8_recipe": "mx"}
 
 
@@ -321,7 +321,7 @@ def create_non_fused_allreduce_gradient_hook(param, accumulation_steps: int, gro
 
 def is_fused_matmul_bias_supported() -> bool:
     """The reference gates ``fused_linear`` on a cuBLASLt-epilogue capability of the Paddle build (sequence_parallel_utils.py:215-220).  Bias
-    (and bias + GELU) always ride in the tcgen05 GEMM epilogue here when the native library is loaded."""
+    (and bias + GELU) always ride in the wgmma GEMM epilogue here when the native library is loaded."""
     from ..ops import _native
 
     return _native.available()

@@ -14,7 +14,7 @@ def check_device(device: str):
     if device in ("gpu", "cuda") and not torch.cuda.is_available():
         raise RuntimeError("Global.device is gpu but no CUDA device is visible; set Global.device=cpu for functional runs")
     if device not in ("gpu", "cuda", "cpu"):
-        raise ValueError(f"unsupported device '{device}': this framework targets NVIDIA B200 (gpu) with a cpu functional path")
+        raise ValueError(f"unsupported device '{device}': this framework targets NVIDIA H100 (gpu) with a cpu functional path")
 
 
 def check_config(cfg):

@@ -296,10 +296,10 @@ _VALID_DEVICES = ("gpu", "cpu")
 
 
 def check_config(cfg: AttrDict) -> None:
-    """One backend (CUDA sm_100a) plus the CPU/gloo correctness path; XPU/NPU/MLU/ROCm dropped."""
+    """One backend (CUDA sm_90a) plus the CPU/gloo correctness path; XPU/NPU/MLU/ROCm dropped."""
     device = str(cfg.Global.get("device", "gpu")).lower()
     if device not in _VALID_DEVICES:
-        raise ValueError(f"device({device}) is not in {list(_VALID_DEVICES)}; this framework targets B200 "
+        raise ValueError(f"device({device}) is not in {list(_VALID_DEVICES)}; this framework targets H100 "
                          "(gpu) with a cpu/gloo path for tests")
     if device == "gpu":
         import torch
@@ -371,7 +371,7 @@ def get_auto_config(fname: str, overrides: Optional[Iterable[str]] = None, show:
         per_gpu = max(lb0 // (int(d0.get("mp_degree", 1) or 1) * int(d0.get("pp_degree", 1) or 1)), 1)
         plans = plan_layouts(ModelShape.from_config(raw), world, per_gpu, top=1)
         if not plans:
-            raise ValueError(f"auto_layout: no layout of this model fits {world} x 180 GB; add GPUs or reduce the batch / sequence length")
+            raise ValueError(f"auto_layout: no layout of this model fits {world} x 80 GB; add GPUs or reduce the batch / sequence length")
         best = plans[0]
         extra = best.overrides() + [f"Global.local_batch_size={per_gpu * best.mp * best.pp * best.cp}", "Global.global_batch_size=None",
                                     "Distributed.auto_layout=False"]

@@ -1,28 +1,27 @@
-"""Auto-parallel planner: choose (dp, sharding + ZeRO stage, mp, pp, micro-batch, recompute) for a transformer on N B200 GPUs.
+"""Auto-parallel planner: choose (dp, sharding + ZeRO stage, mp, pp, micro-batch, recompute) for a transformer on N GPUs.
 
 The reference delegates this to Paddle's static-graph auto-parallel engine: the user writes a process mesh, ``auto.shard_tensor``
 annotations are propagated through the program and an ``OptimizationTuner`` profiles candidates (core/engine/auto_engine.py:39-209,
 models/language_model/gpt/auto/auto_model.py).  In this framework parallelism lives in the layers (``parallel/tp_layers.py``,
 ``pipeline_parallel.py``, the flat ZeRO optimizer), so "auto" means: *search the layout space with a cost model of those concrete
-implementations, keep what fits in 180 GB, rank by predicted step time, and (optionally) measure the top few* — ``AutoEngine`` applies
+implementations, keep what fits in 80 GB, rank by predicted step time, and (optionally) measure the top few* — ``AutoEngine`` applies
 the winner to the config before anything is built.
 
-Cost model (per optimizer step, one GPU's view; every constant is a measurement from ``profiles/`` or ``MEASURED_PEAKS.json``):
+Cost model (per optimizer step, one GPU's view).  The hardware constants are NVIDIA's data-sheet figures for the H100 SXM — nominal, not
+measured; ``MEASURED_PEAKS.json`` at the repository root, when present, replaces the GEMM peak and the HBM bandwidth by measured ones:
 
 * GEMMs — per-GEMM roofline ``max(flops / peak, bytes / hbm) + launch``: tensor parallelism shrinks N or K, sequence parallelism
-  keeps M, so small shards fall off the tensor-core roof by themselves.  ``peak`` = sustained cuBLAS bf16 of MEASURED_PEAKS.json
-  (power-capped B200s sustain ~1.46 PFLOP/s, not the 2.25 nominal); the persistent tcgen05 GEMM measures within a few % of it.
-* attention — flash kernels at their measured rate with dropout (fwd ~315, bwd ~310 TFLOP/s causal, profiles/r2).
-* elementwise / norm / optimizer traffic — bytes over measured HBM copy bandwidth.
-* tensor parallel — 8 collectives per layer per micro-batch of ``tokens x h`` bf16 over NVLink (measured ~620 GB/s per direction);
-  in the full step about one wire time stays exposed with the fused GEMM+collective kernels and 1.6 with NCCL (2-GPU 6.7B runs).
+  keeps M, so small shards fall off the tensor-core roof by themselves.  ``peak`` = dense bf16 tensor rate.
+* attention — causal flash kernels at the tensor rate (an upper bound until they are timed).
+* elementwise / norm / optimizer traffic — bytes over HBM bandwidth.
+* tensor parallel — 8 collectives per layer per micro-batch of ``tokens x h`` bf16 over NVLink (450 GB/s per direction);
+  1.6 wire times are charged as exposed with the fused GEMM+collective kernels and 2.1 with NCCL (assumptions, not H100 measurements).
 * pipeline — 1F1B bubble ``(pp - 1) / (m + pp - 1)`` plus the boundary activations.
-* data parallel / ZeRO — reduce-scatter + all-gather of the local parameters, overlapped with backward / the next forward; what the
-  exposed-communication meter measures at sharding8 (4 ms of a 13 GB exchange) fixes the hidden fraction at 0.9.  Stage 3 adds a
+* data parallel / ZeRO — reduce-scatter + all-gather of the local parameters, overlapped with backward / the next forward; the hidden fraction is taken as 0.9.  Stage 3 adds a
   parameter all-gather per layer per pass.
 
 Memory model: bf16 parameters, gradient buffer, fp32 master + two moments (sharded by ZeRO), activations ``~24 h`` bytes per token
-per layer (calibrated: 6.7B, 8192 tokens, no recompute -> ~20 GB), logits, pipeline in-flight micro-batches, allocator slack.
+per layer, logits, pipeline in-flight micro-batches, allocator slack.
 """
 from __future__ import annotations
 
@@ -31,22 +30,20 @@ import os
 from dataclasses import asdict, dataclass, field
 from typing import Dict, Iterable, List, Optional
 
-HBM_GB = 180.0
+HBM_GB = 80.0
 _REPO = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
 @dataclass
 class Hardware:
-    peak_flops: float = 1.46e15          # sustained bf16 GEMM (cuBLAS, 8192^3, power-capped)
-    hbm_bw: float = 6.5e12               # measured copy bandwidth (read + write bytes)
-    link_bw: float = 6.2e11              # NVLink per direction as our collectives measure it (of 900 GB/s nominal)
-    attn_fwd_flops: float = 3.15e14      # causal flash attention with dropout 0.1 (profiles/r2: 0.218 ms fwd, 0.552 ms bwd at B8 S1024 H32 D128)
-    attn_bwd_flops: float = 3.1e14
+    peak_flops: float = 9.89e14          # dense bf16 tensor rate (H100 SXM data sheet, 700 W; nominal)
+    hbm_bw: float = 3.35e12              # HBM3 bandwidth (data sheet)
+    link_bw: float = 4.5e11              # NVLink 4 per direction (data sheet)
+    attn_fwd_flops: float = 9.89e14      # causal flash attention: the tensor rate as an upper bound, not timed on H100
+    attn_bwd_flops: float = 9.89e14
     launch_s: float = 4e-6
     mem_gb: float = HBM_GB
-    # inside the whole training step the GEMMs run ~7 % below the stand-alone cuBLAS rate: the step sits at the power cap (1.3-1.46 GHz) with
-    # memory-bound kernels in between.  Calibrated on the 1-GPU 6.7B step (313.8 ms, profiles/r2/c14_bench_n1.json)
-    step_efficiency: float = 0.925
+    step_efficiency: float = 1.0         # whole-step derating of the kernel times; 1.0 until a step has been profiled on H100
 
     @staticmethod
     def measured() -> "Hardware":
@@ -169,11 +166,7 @@ def estimate(s: ModelShape, hw: Hardware, world: int, local_batch: int, plan: Pl
     tp = 0.0
     if mp > 1:
         vol = 8.0 * layers_local * tokens * s.hidden * 2.0 * (mp - 1) / mp
-        # exposure calibrated on the 2-GPU 6.7B runs (profiles/r2/bench_c6_mp2_*): +38 ms per step with the fused kernels, +51 ms with NCCL,
-        # for 27.7 ms of wire time — the micro-benchmarks hide 60-70 % of a single collective, the full backward (re-gather + two GEMMs per
-        # collective, smaller N / K) does not
-        # (353 / 367 ms at mp2 against 314 ms on one GPU: 1.6 wire times with the fused kernels, 2.1 with NCCL — this term also carries the
-        # lower efficiency of GEMMs with halved N / K, which the per-GEMM roofline does not see at these sizes)
+        # exposed wire times per collective are assumptions (the full backward re-gathers and runs two smaller GEMMs per collective); not timed on H100
         tp = vol / hw.link_bw * (1.6 if plan.fused_tp else 2.1) + (0 if plan.fused_tp else 8.0 * layers_local * 12e-6)
     if cp > 1 and plan.cp_mode == "ring":
         # ring: (cp - 1) hops per layer of K and V forward (bf16), K / V again plus the fp32 dK / dV accumulators backward = 16 bytes per
@@ -195,12 +188,11 @@ def estimate(s: ModelShape, hw: Hardware, world: int, local_batch: int, plan: Pl
         if stage == 3:
             dp_comm += 2.0 * n_micro * p_local * 2.0 * (sd - 1) / sd / hw.link_bw     # per-layer gathers in forward and backward
     # 10 % of the exchange is exposed outright (first / last bucket); the hidden 90 % still costs about half its duration because the
-    # collective kernels take SMs, HBM bandwidth and power from the GEMMs they run beside (sharding8: 325 ms vs 314 ms on one GPU with an
-    # optimizer 8x smaller — profiles/r2/c15_bench_n8.json)
+    # collective kernels take SMs and HBM bandwidth from the GEMMs they run beside (an assumption, not timed on H100)
     exposed_dp = (0.1 + 0.5) * dp_comm + (0.0 if data_ranks == 1 else 1.5e-3)
     # AdamW over the local shard: 2 (bf16 w) + 4 (grad) + 12 (master, m, v read) + 12 (write) bytes per parameter; overlapped with the next forward
     opt = p_local / (sd if stage >= 1 else 1) * 30.0 / hw.hbm_bw
-    exposed_opt = 0.6 * opt            # "overlapped" still costs: the forward GEMMs it runs beside slow down 2-3x (trace, profiles/r2)
+    exposed_opt = 0.6 * opt            # "overlapped" still costs: the forward GEMMs it runs beside slow down
     step = compute + bubble + exposed_dp + exposed_opt
     # ---- memory
     shard = sd if stage >= 1 else 1

@@ -150,8 +150,8 @@ class Logger:
 
 def advertise() -> None:
     """Banner shown above the config dump (reference: utils/log.py advertise())."""
-    title = "PaddleFleetX-B200"
-    sub = "Blackwell-native large-model training suite"
+    title = "PaddleFleetX-H100"
+    sub = "Hopper-native (H100) large-model training suite"
     width = max(len(title), len(sub)) + 8
     bar = "=" * width
     logger.info(bar)

@@ -4,7 +4,7 @@
 B200-first design: the primary signal is *device time per kernel* from CUPTI via ``torch.profiler`` restricted to the scheduled
 step window, plus NVTX ranges (``torch.cuda.nvtx``) around every step so that an external ``ncu --nvtx`` capture can be aligned
 with the same window.  The summary is written both as a chrome trace and as a flat per-kernel table (json) under
-``profiler_log`` — the table is what ``profiles/`` summaries are generated from.
+``profiler_log``.
 """
 from __future__ import annotations
 

@@ -12,6 +12,6 @@ def version_check():
         raise RuntimeError(f"paddlefleetx_b200 needs torch >= {MIN_TORCH[0]}.{MIN_TORCH[1]}, found {torch.__version__}")
     if torch.cuda.is_available():
         major, minor = torch.cuda.get_device_capability()
-        if (major, minor) != (10, 0):
-            logger.warning(f"kernels are built for sm_100a only; this device is sm_{major}{minor} — native ops will refuse to load")
+        if (major, minor) != (9, 0):
+            logger.warning(f"kernels are built for sm_90a only; this device is sm_{major}{minor} — native ops will refuse to load")
     return True

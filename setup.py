@@ -1,4 +1,4 @@
-"""``pip install -e .`` builds the sm_100a kernel library and the C++ dataset helper in-tree (reference setup.py:17-38 runs the C++
+"""``pip install -e .`` builds the sm_90a kernel library and the C++ dataset helper in-tree (reference setup.py:17-38 runs the C++
 ``make`` at install time and ships ``fast_index_map_helpers.so`` as package data)."""
 import os
 import subprocess
@@ -18,7 +18,7 @@ class BuildNative(build_py):
 setup(
     name="paddlefleetx_b200",
     version="0.1.0",
-    description="B200-native large-model training and serving framework (GPT / ERNIE / MoE / ViT / MoCo / Imagen recipes)",
+    description="H100 (sm_90a) large-model training and serving framework (GPT / ERNIE / MoE / ViT / MoCo / Imagen recipes)",
     packages=find_packages(include=["paddlefleetx_b200", "paddlefleetx_b200.*", "ppfleetx", "ppfleetx.*"]),
     package_data={"paddlefleetx_b200": ["configs/**/*.yaml", "ops/*.so", "ops/csrc/*", "data/data_tools/cpp/*"]},
     python_requires=">=3.10",

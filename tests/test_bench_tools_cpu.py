@@ -32,8 +32,8 @@ def test_analyze_trace_interval_arithmetic_and_report(tmp_path, capsys):
     assert A.total([[0, 3], [5, 8]]) == 6
     assert A.intersect([[0, 3], [5, 8]], [[2, 6], [7, 9]]) == 1 + 1 + 1
     trace = {"steps": 2, "model": "toy", "n_gpus": 1, "columns": ["name", "stream", "ts_us", "dur_us"],
-             "kernels": [["void pfx::gemm_tcgen05_kernel<2, 256>", 7, 0.0, 100.0], ["pfx::(anonymous namespace)::adamw_flat_kernel", 9, 50.0, 100.0],
-                         ["void pfx::gemm_tcgen05_kernel<2, 256>", 7, 200.0, 100.0], ["ncclDevKernel_ReduceScatter", 9, 250.0, 100.0]]}
+             "kernels": [["void pfx::gemm_wgmma_kernel<128>", 7, 0.0, 100.0], ["pfx::(anonymous namespace)::adamw_flat_kernel", 9, 50.0, 100.0],
+                         ["void pfx::gemm_wgmma_kernel<128>", 7, 200.0, 100.0], ["ncclDevKernel_ReduceScatter", 9, 250.0, 100.0]]}
     path = tmp_path / "t.json.gz"
     with gzip.open(path, "wt") as f:
         json.dump(trace, f)
@@ -44,7 +44,7 @@ def test_analyze_trace_interval_arithmetic_and_report(tmp_path, capsys):
     finally:
         sys.argv = old
     out = capsys.readouterr().out
-    assert "4 kernels over 2 steps" in out and "gemm_tcgen05_kernel" in out
+    assert "4 kernels over 2 steps" in out and "gemm_wgmma_kernel" in out
 
 
 def test_reference_arm_reports_unavailable_and_exits_zero():

@@ -1,5 +1,5 @@
 """The user-facing command line, end to end, as subprocesses: train (with checkpoint) -> resume -> generate -> export -> serve ->
-latency tool.  Runs on CPU in the default suite and on the B200 with ``-m gpu`` (bf16, native kernels, CUDA-graph decode)."""
+latency tool.  Runs on CPU in the default suite and on the H100 with ``-m gpu`` (bf16, native kernels, CUDA-graph decode)."""
 import os
 import re
 import subprocess

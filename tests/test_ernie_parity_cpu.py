@@ -1,17 +1,18 @@
 """ERNIE parity: ``ErnieForPretraining(ErnieModel(..))`` and the sequence-classification head built by the REFERENCE constructors
 (ernie/dygraph/single_model.py + ernie/layers/transformer.py, executed unmodified on a ``paddle.nn`` -> ``torch.nn`` shim, meta device) and by
-ours have the same number of parameters and the same multiset of tensor sizes.  Skipped when /root/reference is absent."""
+ours have the same number of parameters and the same multiset of tensor sizes.  The original constructors are replayed from tests/golden (see golden_ref.py)."""
+import contextlib
 import importlib
 import os
 import sys
 import types
 
+import golden_ref
 import pytest
 import torch
 import torch.nn as tnn
 
-REF_DIR = "/root/reference/ppfleetx/models/language_model/ernie"
-pytestmark = pytest.mark.skipif(not os.path.isfile(os.path.join(REF_DIR, "dygraph", "single_model.py")), reason="reference tree not available")
+REF_DIR = os.path.join(golden_ref.REFERENCE_DIR, "ppfleetx/models/language_model/ernie")
 
 CONFIGS = {"base": dict(vocab_size=40000, hidden_size=768, num_hidden_layers=12, num_attention_heads=12, intermediate_size=3072, max_position_embeddings=512, type_vocab_size=4),
            "large": dict(vocab_size=40000, hidden_size=1024, num_hidden_layers=24, num_attention_heads=16, intermediate_size=4096, max_position_embeddings=512, type_vocab_size=4),
@@ -90,8 +91,8 @@ def _shim():
     return m
 
 
-@pytest.fixture(scope="module")
-def ref_ernie():
+@contextlib.contextmanager
+def _load_reference():
     mods = _shim()
     saved = {k: sys.modules.get(k) for k in mods}
     sys.modules.update(mods)
@@ -108,6 +109,12 @@ def ref_ernie():
                 sys.modules[k] = v
         for k in [k for k in sys.modules if k.startswith("_ref_ernie")]:
             sys.modules.pop(k, None)
+
+
+@pytest.fixture(scope="module")
+def ref_ernie():
+    with golden_ref.namespaces("ernie_parity", _load_reference) as (ns,):
+        yield ns
 
 
 def _sizes(m):

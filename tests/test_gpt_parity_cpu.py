@@ -1,17 +1,18 @@
 """GPT parity: ``GPTModel`` / ``GPTForPretraining`` built by the REFERENCE constructor (gpt/dygraph/single_model.py, executed unmodified on a
 ``paddle.nn`` -> ``torch.nn`` shim, meta device) and by ours must have the same number of parameters and the same multiset of tensor sizes, for
-the published model sizes (345M ... 175B) with and without the fused QKV projection.  Skipped when /root/reference is absent."""
+the published model sizes (345M ... 175B) with and without the fused QKV projection.  The original constructors are replayed from tests/golden (see golden_ref.py)."""
+import contextlib
 import importlib
 import os
 import sys
 import types
 
+import golden_ref
 import pytest
 import torch
 import torch.nn as tnn
 
-REF_DIR = "/root/reference/ppfleetx/models/language_model/gpt/dygraph"
-pytestmark = pytest.mark.skipif(not os.path.isfile(os.path.join(REF_DIR, "single_model.py")), reason="reference tree not available")
+REF_DIR = os.path.join(golden_ref.REFERENCE_DIR, "ppfleetx/models/language_model/gpt/dygraph")
 
 SIZES = {"345M": (24, 1024, 16), "1.3B": (24, 2048, 16), "6.7B": (32, 4096, 32), "13B": (40, 5120, 40), "175B": (96, 12288, 96)}
 
@@ -78,8 +79,8 @@ def _shim():
     return m
 
 
-@pytest.fixture(scope="module")
-def ref_gpt():
+@contextlib.contextmanager
+def _load_reference():
     import ppfleetx.models.language_model.moe  # noqa: F401  (imported by the reference file through the alias package; not constructed here)
     import ppfleetx.models.language_model.moe_exp.layer  # noqa: F401
     import ppfleetx.utils.log  # noqa: F401
@@ -97,6 +98,12 @@ def ref_gpt():
                 sys.modules[k] = v
         for k in [k for k in sys.modules if k.startswith("_ref_gpt")]:
             sys.modules.pop(k, None)
+
+
+@pytest.fixture(scope="module")
+def ref_gpt():
+    with golden_ref.namespaces("gpt_parity", _load_reference) as (ns,):
+        yield ns
 
 
 def _sizes(m):

@@ -1,4 +1,4 @@
-"""Model families on a real B200: every zoo member runs forward + backward + optimizer step in bf16 on CUDA through the native
+"""Model families on a real H100: every zoo member runs forward + backward + optimizer step in bf16 on CUDA through the native
 op layer (the CPU suite only exercises the PyTorch expressions), and the serving / parallel-free engine paths work end to end."""
 import os
 
@@ -139,7 +139,7 @@ def test_int8_serving_conversion_on_gpu():
     assert quantize_tp_linears_int8(q) == 8
     ids = torch.arange(1, 41, device="cuda").view(1, 40)
     with torch.no_grad():
-        for n in (1, 3, 40):                    # W8A8 GEMV (<= 8 rows) and the tcgen05 int8 GEMM
+        for n in (1, 3, 40):                    # W8A8 GEMV (<= 8 rows) and the wgmma int8 GEMM
             a, b = ref(ids[:, :n]).float(), q(ids[:, :n]).float()
             assert float((a - b).norm() / a.norm()) < 0.05, n
 
@@ -227,7 +227,7 @@ def test_ernie_trains_on_gpu(tmp_path):
 
 
 def test_native_flash_attention_serves_inference_and_training():
-    """attention() routes unmasked bf16 calls (head dim 64 / 128) to the tcgen05 flash kernels: forward without grad, forward + backward with
+    """attention() routes unmasked bf16 calls (head dim 64 / 128) to the wgmma flash kernels: forward without grad, forward + backward with
     grad (no library kernel), a masked call falls back to SDPA; all three match fp32."""
     import torch.nn.functional as F
 
@@ -263,7 +263,7 @@ def test_native_flash_attention_serves_inference_and_training():
 
 def test_evoformer_block_runs_on_the_native_attention_kernels(monkeypatch):
     """One Evoformer iteration at the production head geometry (c_m 256 / 8 heads, c_z 128 / 4 heads: 32-wide heads) in bf16: every gated
-    attention (MSA row with pair bias, MSA column, triangle start / end) goes through csrc/evoformer_attn_sm100.cu forward AND backward, and
+    attention (MSA row with pair bias, MSA column, triangle start / end) goes through csrc/evoformer_attn_sm90.cu forward AND backward, and
     agrees with the plain PyTorch expression."""
     from paddlefleetx_b200.models.protein_folding.evoformer import EvoformerIteration
     from paddlefleetx_b200.ops import evoformer_attention as EA

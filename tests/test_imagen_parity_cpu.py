@@ -1,17 +1,18 @@
 """Imagen U-Net parity: the four presets (and a sweep of constructor options) must build networks with exactly the parameter
 count of the REFERENCE constructors.  The reference sources are executed unmodified for their ``__init__`` only, on top of a few-line
-``paddle.nn`` -> ``torch.nn`` shim on the meta device (no Paddle needed, no memory allocated); skipped when /root/reference is absent."""
+``paddle.nn`` -> ``torch.nn`` shim on the meta device (no Paddle needed, no memory allocated); the original constructors are replayed from tests/golden (see golden_ref.py)."""
+import contextlib
 import importlib
 import os
 import sys
 import types
 
+import golden_ref
 import pytest
 import torch
 import torch.nn as tnn
 
-REF_DIR = "/root/reference/ppfleetx/models/multimodal_model/imagen"
-pytestmark = pytest.mark.skipif(not os.path.isfile(os.path.join(REF_DIR, "unet.py")), reason="reference tree not available")
+REF_DIR = os.path.join(golden_ref.REFERENCE_DIR, "ppfleetx/models/multimodal_model/imagen")
 
 
 def _install_shim():
@@ -49,8 +50,8 @@ def _install_shim():
     return mods
 
 
-@pytest.fixture(scope="module")
-def ref_unet():
+@contextlib.contextmanager
+def _load_reference():
     import ppfleetx.models.language_model  # noqa: F401  (the alias package must be importable before its t5 leaf is stubbed)
 
     mods = _install_shim()
@@ -74,6 +75,12 @@ def ref_unet():
                 sys.modules[k] = v
         for k in [k for k in sys.modules if k.startswith("_ref_imagen")]:
             sys.modules.pop(k, None)
+
+
+@pytest.fixture(scope="module")
+def ref_unet():
+    with golden_ref.namespaces("imagen_parity", _load_reference, count=2) as nss:
+        yield tuple(nss)
 
 
 def _count(m):

@@ -8,7 +8,7 @@ from paddlefleetx_b200.utils import config as C
 from paddlefleetx_b200.utils.layout_planner import Hardware, ModelShape, Plan, estimate, plan_layouts
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GPT = {"345m": (24, 1024, 16), "6.7b": (32, 4096, 32), "13b": (40, 5120, 40), "175b": (96, 12288, 96)}
+GPT = {"345m": (24, 1024, 16), "1.3b": (24, 2048, 16), "6.7b": (32, 4096, 32), "13b": (40, 5120, 40), "175b": (96, 12288, 96)}
 
 
 def shape(name, seq=1024):
@@ -35,13 +35,14 @@ def test_6p7b_prefers_zero_sharding_over_tensor_parallel_on_one_node():
 
 def test_memory_forces_model_parallelism_and_recompute():
     hw = Hardware()
-    assert plan_layouts(shape("175b"), 8, 1, hw=hw) == []          # 175B x 16+ bytes does not fit 8 x 180 GB in any layout
+    assert plan_layouts(shape("175b"), 8, 1, hw=hw) == []          # 175B x 16+ bytes does not fit 8 x 80 GB in any layout
     plans = plan_layouts(shape("175b"), 64, 1, hw=hw)
     assert plans and all(p.mp * p.pp * (p.sharding if p.stage >= 2 else 1) >= 8 for p in plans[:3])
-    one = plan_layouts(shape("6.7b"), 1, 8, hw=hw)
-    assert one and one[0].est_mem_gb < 0.92 * 180
-    big_batch = plan_layouts(shape("6.7b"), 1, 32, hw=hw)           # 32 k tokens of activations on top of 120 GB of states: recompute or smaller micro-batch
-    assert big_batch and (big_batch[0].recompute != "none" or big_batch[0].micro_batch < 32)
+    assert plan_layouts(shape("6.7b"), 1, 8, hw=hw) == []           # 106 GB of weights + AdamW state: not on one 80 GB GPU
+    one = plan_layouts(shape("1.3b"), 1, 8, hw=hw)
+    assert one and one[0].est_mem_gb < 0.92 * 80
+    big_batch = plan_layouts(shape("1.3b"), 1, 64, hw=hw)           # 64 k tokens of activations on top of the states: recompute or smaller micro-batch
+    assert big_batch and (big_batch[0].recompute != "none" or big_batch[0].micro_batch < 64)
 
 
 def test_estimates_are_monotonic():
@@ -74,14 +75,14 @@ def test_long_sequences_bring_in_context_parallelism():
     hw = Hardware()
     s = ModelShape(layers=40, hidden=5120, heads=40, vocab=50304, ffn=20480, seq=32768)
     plans = plan_layouts(s, 8, 1, hw=hw)
-    assert plans and plans[0].cp > 1 and plans[0].est_mem_gb < 0.92 * 180
+    assert plans and plans[0].cp > 1 and plans[0].est_mem_gb < 0.92 * 80
     no_cp = [p for p in plans if p.cp == 1 and p.mp == 1 and p.pp == 1]
     assert all(p.recompute != "none" or p.stage == 3 for p in no_cp[:1]) or not no_cp       # without cp it needs recompute / stage 3 (or does not fit)
     assert "Distributed.cp_degree=%d" % plans[0].cp in plans[0].overrides()
     assert all(p.cp == 1 for p in plan_layouts(shape("6.7b"), 8, 8, hw=hw))
     # same tokens per GPU per step with and without cp
     a = next(p for p in plans if p.cp == 2)
-    assert a.micro_batch * a.accumulate == 2
+    assert a.micro_batch * a.accumulate == 2 * a.mp * a.pp           # one sequence per GPU of the data rank's cp x mp x pp group
 
 
 def test_ring_mode_covers_head_counts_ulysses_cannot_split_and_hides_its_transfers():
@@ -100,20 +101,17 @@ def test_ring_mode_covers_head_counts_ulysses_cannot_split_and_hides_its_transfe
     assert ring.breakdown["tp_comm"] <= uly.breakdown["tp_comm"] and "ring" in ring.describe()
 
 
-def test_cost_model_reproduces_the_measured_6p7b_layouts():
-    """The five GPT-6.7B layouts measured on B200s in round 2 (profiles/r2: c14_bench_n1, c15_bench_n8 + its named_layout, bench_c6_mp2_*): the
-    default hardware constants predict each step within 4 %, and rank them in the measured order."""
-    s, hw = shape("6.7b"), Hardware()
+def test_cost_model_ranks_the_6p7b_layouts():
+    """No step of these layouts has been timed on H100, so the defaults (data-sheet constants) are held to properties only: ZeRO sharding costs
+    more than one GPU's step, tensor parallelism more than sharding, NCCL more than the fused kernels, the pipelined layout most."""
+    s, hw = shape("6.7b"), Hardware(mem_gb=1e9)
     base = dict(dp=1, sharding=1, stage=1, mp=1, pp=1, micro_batch=8, accumulate=1, recompute="none", sequence_parallel=False, fused_tp=False)
-    cases = [  # world, sequences per data rank, plan, measured ms / step
-        (1, 8, dict(), 313.8),
-        (8, 8, dict(sharding=8), 325.1),
-        (2, 16, dict(mp=2, micro_batch=16, sequence_parallel=True, fused_tp=True), 353.2),
-        (2, 16, dict(mp=2, micro_batch=16, sequence_parallel=True, fused_tp=False), 366.9),
-        (8, 32, dict(mp=2, pp=2, sharding=2, micro_batch=4, accumulate=8, sequence_parallel=True, fused_tp=True), 448.0)]
-    pred = []
-    for world, lb, kw, measured in cases:
-        p = estimate(s, hw, world, lb, Plan(**{**base, **kw}))
-        assert abs(p.est_step_s * 1e3 / measured - 1.0) < 0.04, (kw, p.est_step_s * 1e3, measured)
-        pred.append(p.est_step_s)
-    assert pred == sorted(pred)
+    cases = [  # world, sequences per data rank, plan
+        (1, 8, dict()),
+        (8, 8, dict(sharding=8)),
+        (2, 16, dict(mp=2, micro_batch=16, sequence_parallel=True, fused_tp=True)),
+        (2, 16, dict(mp=2, micro_batch=16, sequence_parallel=True, fused_tp=False)),
+        (8, 32, dict(mp=2, pp=2, sharding=2, micro_batch=4, accumulate=8, sequence_parallel=True, fused_tp=True))]
+    pred = [estimate(s, hw, world, lb, Plan(**{**base, **kw})).est_step_s for world, lb, kw in cases]
+    assert pred == sorted(pred) and len(set(pred)) == len(pred)
+    assert Hardware().peak_flops == 9.89e14 and Hardware().hbm_bw == 3.35e12 and Hardware().link_bw == 4.5e11 and Hardware().mem_gb == 80.0

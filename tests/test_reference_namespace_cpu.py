@@ -2,21 +2,40 @@
 defines at module level exist in ours.  This is the "switch the import and keep going" contract of the ``ppfleetx`` alias package."""
 import ast
 import importlib
+import json
 import os
 
-import pytest
+import golden_ref
 
-REF = "/root/reference/ppfleetx"
-pytestmark = pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not present")
+GOLDEN = os.path.join(golden_ref.GOLDEN_DIR, "reference_namespace.json")      # {module name below ppfleetx: "public names"}
+_SKIP_PREFIX = ("_",)
+
+
+def _public_defs(path):
+    tree = ast.parse(open(path, encoding="utf-8").read())
+    out = []
+    for node in tree.body:
+        if isinstance(node, (ast.ClassDef, ast.FunctionDef)) and not node.name.startswith(_SKIP_PREFIX):
+            out.append(node.name)
+    return out
 
 
 def _reference_modules():
-    for dirpath, _, files in os.walk(REF):
+    """(module name, public names) of every module of the original package: from the stored list, or from a checkout (which rewrites the list)."""
+    if not golden_ref.REFERENCE_DIR:
+        with open(GOLDEN, encoding="utf-8") as f:
+            return sorted((("ppfleetx." + k).rstrip("."), v.split()) for k, v in json.load(f).items())
+    ref, found = os.path.join(golden_ref.REFERENCE_DIR, "ppfleetx"), {}
+    for dirpath, _, files in os.walk(ref):
         for f in sorted(files):
             if f.endswith(".py"):
-                rel = os.path.relpath(os.path.join(dirpath, f), os.path.dirname(REF))[:-3]
+                rel = os.path.relpath(os.path.join(dirpath, f), os.path.dirname(ref))[:-3]
                 name = rel.replace(os.sep, ".")
-                yield (name[:-len(".__init__")] if name.endswith(".__init__") else name), os.path.join(dirpath, f)
+                found[name[:-len(".__init__")] if name.endswith(".__init__") else name] = _public_defs(os.path.join(dirpath, f))
+    with open(GOLDEN, "w", encoding="utf-8") as f:
+        json.dump({k[len("ppfleetx"):].lstrip("."): " ".join(v) for k, v in found.items()}, f, separators=(",", ":"), sort_keys=True)
+        f.write("\n")
+    return sorted(found.items())
 
 
 def test_every_reference_module_name_imports():
@@ -32,7 +51,6 @@ def test_every_reference_module_name_imports():
     assert not missing, "\n".join(missing)
 
 
-_SKIP_PREFIX = ("_",)
 # public names of the reference not provided yet, one ``module.name`` per line; the test fails when a name outside this file goes missing AND
 # when a listed name has been provided (so the file can only shrink)
 _KNOWN_GAPS_FILE = os.path.join(os.path.dirname(__file__), "reference_namespace_known_gaps.txt")
@@ -45,24 +63,15 @@ def _known_gaps():
         return {line.strip() for line in f if line.strip() and not line.startswith("#")}
 
 
-def _public_defs(path):
-    tree = ast.parse(open(path, encoding="utf-8").read())
-    out = []
-    for node in tree.body:
-        if isinstance(node, (ast.ClassDef, ast.FunctionDef)) and not node.name.startswith(_SKIP_PREFIX):
-            out.append(node.name)
-    return out
-
-
 def test_public_classes_and_functions_exist():
     absent = set()
     total = 0
-    for name, path in _reference_modules():
+    for name, defs in _reference_modules():
         try:
             mod = importlib.import_module(name)
         except Exception:               # noqa: BLE001 - reported by the test above
             continue
-        for sym in _public_defs(path):
+        for sym in defs:
             total += 1
             if not hasattr(mod, sym):
                 absent.add(f"{name}.{sym}")

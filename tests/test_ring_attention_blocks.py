@@ -1,6 +1,6 @@
 """The block schedule of parallel/ring_attention.py replayed inside ONE process (every "rank" is a zigzag slice of the same tensors, the ring
 hop is a list rotation): checks the block plan, the online-softmax merge and the backward-from-final-statistics against attention over the whole
-sequence.  On CPU it runs the PyTorch block; the ``gpu`` variant runs the same schedule through the tcgen05 flash kernels in bf16 — the block
+sequence.  On CPU it runs the PyTorch block; the ``gpu`` variant runs the same schedule through the wgmma flash kernels in bf16 — the block
 shapes a ring produces (``q x k[:half]``, ``q[half:] x k``, unmasked, statistics of the FULL row) are shapes no other test feeds them."""
 import pytest
 import torch

@@ -1,17 +1,18 @@
 """Text-tower parity (Imagen's encoders): ``T5EncoderModel`` built by the REFERENCE constructor (language_model/t5/modeling.py, executed
 unmodified on a ``paddle.nn`` -> ``torch.nn`` shim, meta device) and by ours must have the same parameter count and the same multiset of tensor
-sizes, for t5-11b and smaller shapes.  Skipped when /root/reference is absent."""
+sizes, for t5-11b and smaller shapes.  The original constructors are replayed from tests/golden (see golden_ref.py)."""
+import contextlib
 import importlib
 import os
 import sys
 import types
 
+import golden_ref
 import pytest
 import torch
 import torch.nn as tnn
 
-REF = "/root/reference/ppfleetx/models/language_model"
-pytestmark = pytest.mark.skipif(not os.path.isfile(os.path.join(REF, "t5", "modeling.py")), reason="reference tree not available")
+REF = os.path.join(golden_ref.REFERENCE_DIR, "ppfleetx/models/language_model")
 
 
 def _shim():
@@ -59,8 +60,8 @@ def _shim():
     return m
 
 
-@pytest.fixture(scope="module")
-def ref_t5():
+@contextlib.contextmanager
+def _load_reference():
     import ppfleetx.data.tokenizers.t5_tokenizer  # noqa: F401  (imported by the reference module through the alias package)
     import ppfleetx.models.multimodal_model.imagen.utils  # noqa: F401
 
@@ -77,6 +78,12 @@ def ref_t5():
                 sys.modules[k] = v
         for k in [k for k in sys.modules if k.startswith("_ref_lm")]:
             sys.modules.pop(k, None)
+
+
+@pytest.fixture(scope="module")
+def ref_t5():
+    with golden_ref.namespaces("t5_parity", _load_reference, names=True) as (ns,):
+        yield ns
 
 
 def _sizes(m):

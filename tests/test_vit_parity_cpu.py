@@ -1,18 +1,19 @@
 """ViT parity: every preset (tiny ... 6B) must build a network with exactly the parameter count — and the same per-tensor shapes — as the
 REFERENCE constructor.  The reference sources (vision_model/vit/vit.py and vision_model/layers/*.py) are executed unmodified for their
-``__init__`` on top of a small ``paddle.nn`` -> ``torch.nn`` shim on the meta device; skipped when /root/reference is absent."""
+``__init__`` on top of a small ``paddle.nn`` -> ``torch.nn`` shim on the meta device; the original constructors are replayed from tests/golden (see golden_ref.py)."""
+import contextlib
 import importlib
 import os
 import sys
 import types
 from collections import Counter
 
+import golden_ref
 import pytest
 import torch
 import torch.nn as tnn
 
-REF_DIR = "/root/reference/ppfleetx/models/vision_model"
-pytestmark = pytest.mark.skipif(not os.path.isfile(os.path.join(REF_DIR, "vit", "vit.py")), reason="reference tree not available")
+REF_DIR = os.path.join(golden_ref.REFERENCE_DIR, "ppfleetx/models/vision_model")
 
 PRESETS = ["ViT_tiny_patch16_224", "ViT_base_patch16_224", "ViT_base_patch16_384", "ViT_base_patch32_224", "ViT_base_patch32_384",
            "ViT_large_patch16_224", "ViT_large_patch16_384", "ViT_large_patch32_224", "ViT_large_patch32_384", "ViT_huge_patch14_224",
@@ -71,8 +72,8 @@ def _shim():
             "paddle.incubate.nn": inc_nn, "_ref_vis": pkg, "_ref_vis.vit": vit_pkg, "_ref_vis.layers": layers_pkg}
 
 
-@pytest.fixture(scope="module")
-def ref_vit():
+@contextlib.contextmanager
+def _load_reference():
     import ppfleetx.utils.log  # noqa: F401  (the reference file imports the logger through the alias package)
 
     mods = _shim()
@@ -88,6 +89,12 @@ def ref_vit():
                 sys.modules[k] = v
         for k in [k for k in sys.modules if k.startswith("_ref_vis")]:
             sys.modules.pop(k, None)
+
+
+@pytest.fixture(scope="module")
+def ref_vit():
+    with golden_ref.namespaces("vit_parity", _load_reference) as (ns,):
+        yield ns
 
 
 def _shapes(m):

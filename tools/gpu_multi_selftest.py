@@ -319,7 +319,7 @@ def finish(res, rank, world):
 
 def nvls_section(lib, grp, rank, world, report):
     """Symmetric memory on cuMem VMM, multicast (NVLS) and unicast variants of the ZeRO kernels against NCCL, and the experiment the
-    design rests on: does a communication kernel overlap with a stream of persistent tcgen05 GEMMs, or serialise with it?"""
+    design rests on: does a communication kernel overlap with a stream of persistent wgmma GEMMs, or serialise with it?"""
     from paddlefleetx_b200.parallel.symmetric_memory import VmmSymmetricAllocator
 
     caps = lib.vmm_caps()
@@ -359,7 +359,7 @@ def nvls_section(lib, grp, rank, world, report):
         e2 = relerr(o32 - 1.0, ref.float() * 0.5)
         report(f"symm_reduce_scatter_{name}_f32acc", err=e2, ok=e2 < 1e-2)
         perf = {}
-        for ctas in (16, 32, 64, 128, 296):
+        for ctas in (16, 32, 64, 128, 264):
             perf[str(ctas)] = timed(lambda: (sm.barrier(), lib.symm_reduce_scatter(mcp, peers, rank * n, out, rank, 1, 1.0, False, None, ctas)))
         best = min(perf.values())
         report(f"symm_reduce_scatter_{name}_perf", ms_by_ctas=perf, nccl_ms=t_nccl, shard_mib=n * 2 / 2 ** 20,
@@ -395,11 +395,11 @@ def nvls_section(lib, grp, rank, world, report):
         ref_full = torch.empty(n * world, dtype=torch.bfloat16, device="cuda")
         dist.all_gather_into_tensor(ref_full, ref_lp)
         torch.cuda.synchronize(); sm.barrier()
-        lib.adamw_symm_broadcast_(sm.mc_ptr(pfull) if mcp else 0, sm.peer_ptrs(pfull), rank * n, master, g, m0, v0, 1e-3, 0.9, 0.999, 1e-8, 0.01, 1, gs, fi, 1, rank, 296)
+        lib.adamw_symm_broadcast_(sm.mc_ptr(pfull) if mcp else 0, sm.peer_ptrs(pfull), rank * n, master, g, m0, v0, 1e-3, 0.9, 0.999, 1e-8, 0.01, 1, gs, fi, 1, rank, 264)
         sm.barrier(); torch.cuda.synchronize()
         ok = bool(torch.equal(pfull, ref_full)) and bool(torch.equal(master, ref_master))
         t = timed(lambda: (lib.adamw_symm_broadcast_(sm.mc_ptr(pfull) if mcp else 0, sm.peer_ptrs(pfull), rank * n, master, g, m0, v0, 1e-3, 0.9, 0.999,
-                                                     1e-8, 0.01, 2, gs, fi, 1, rank, 296), sm.barrier()))
+                                                     1e-8, 0.01, 2, gs, fi, 1, rank, 264), sm.barrier()))
         t_ref = timed(lambda: (lib.adamw_flat_(ref_lp, ref_master, g, ref_m, ref_v, 1e-3, 0.9, 0.999, 1e-8, 0.01, 2, gs, fi),
                                dist.all_gather_into_tensor(ref_full, ref_lp)))
         report(f"adamw_symm_broadcast_{name}", ok=ok, ms=t, adamw_plus_nccl_ag_ms=t_ref, shard_melems=n / 1e6)
@@ -445,7 +445,7 @@ def nvls_section(lib, grp, rank, world, report):
 
     t_g = timed(gemms, iters=3, warmup=1)
     res_ov = {"gemm_only_ms": t_g, "n_gemm": n_gemm, "bucket_mib": n * world * 4 / 2 ** 20, "reps": reps}
-    for ctas in (32, 64, 148):
+    for ctas in (32, 64, 132):
         res_ov[f"ours{ctas}_only_ms"] = timed(comm_ours(ctas), iters=3, warmup=1)
         res_ov[f"ours{ctas}_both_ms"] = timed(both(comm_ours(ctas)), iters=3, warmup=1)
     res_ov["nccl_only_ms"] = timed(comm_nccl, iters=3, warmup=1)

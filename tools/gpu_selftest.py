@@ -1,4 +1,4 @@
-"""Stand-alone numerics + timing sweep of the native kernels on one B200.
+"""Stand-alone numerics + timing sweep of the native kernels on one H100.
 
 Each check runs in its own subprocess under a timeout so that a hung or trapping kernel cannot take the whole
 sweep (or the GPU box) down.  Results are appended to ``gpurun_out/selftest.log`` as JSON lines.
@@ -294,7 +294,7 @@ def check_gemv():
         med_c, _ = _time(lambda: torch.nn.functional.linear(x, w, b))
         med_t, _ = _time(lambda: lib.gemm(x, w, b, None, True, True, 1, 0, 0))
         res[f"{M}x{N}x{K}"] = dict(err=round(e, 5), ms=round(med, 4), gbs=round(N * K * 2 / med / 1e6, 1), cublas_ms=round(med_c, 4),
-                                   tcgen05_gemm_ms=round(med_t, 4))
+                                   wgmma_gemm_ms=round(med_t, 4))
     return dict(ok=ok, shapes=res)
 
 
@@ -720,22 +720,8 @@ def check_norm_residual():
     return dict(ok=ok, cases=res)
 
 
-def check_probe_tmem_a():
-    """tcgen05.mma with the A operand in tensor memory (packed there by tcgen05.st, one row per lane) == A . B^T."""
-    import torch
-    lib = _lib()
-    torch.manual_seed(0)
-    a = torch.randn(128, 128, device="cuda").bfloat16()
-    b = torch.randn(64, 128, device="cuda").bfloat16()
-    d = lib.probe_tmem_a(a, b)
-    torch.cuda.synchronize()
-    ref = a.float() @ b.float().t()
-    err = _relerr(d, ref)
-    return dict(ok=bool(err < 1e-3), err=err)
-
-
 def check_gemm_big_sweep():
-    """Multi-tile shapes (several tiles per CTA, both TMEM accumulator buffers alternating, dozens of k-blocks, ragged edges) for every
+    """Multi-tile shapes (several tiles per CTA, dozens of k-blocks, ragged edges) for every
     (CTA-group, operand majors, output mode) against fp32."""
     worst, rows, ok = 0.0, {}, True
     for cfg in (1, 2, 3, 4):
@@ -934,7 +920,7 @@ def _mx_encode_sf(e_rows_kb):
 
 
 def check_gemm_mxfp8(perf=False):
-    """MX block-scaled fp8 GEMM (kind::mxf8f6f4.block_scale, scales through TMEM) in stages that isolate each piece of the protocol: unit
+    """MX block-scaled fp8 GEMM in stages that isolate each piece of the protocol: unit
     scales, per-row A scales (lane / column mapping), per-K-block scales (sf_id), B scales, then quantiser + GEMM against fp32."""
     import torch
     lib = _lib()
@@ -1027,7 +1013,6 @@ CHECKS = {
     "attention_autograd": check_attention_autograd,
     "gemm_big_sweep": check_gemm_big_sweep,
     "embedding": check_embedding,
-    "probe_tmem_a": check_probe_tmem_a,
     "norm_residual": check_norm_residual,
     "attention_decode": check_attention_decode,
     "gemv_w8a8": check_gemv_w8a8,

@@ -1,6 +1,6 @@
 """Environment validation (the reference tells users to run ``paddle.utils.run_check()`` and a launcher check — docs/deployment_faq.md:75,107):
 
-    python tools/run_check.py                 # this process: CUDA device, sm_100a, native library, one tcgen05 GEMM vs PyTorch
+    python tools/run_check.py                 # this process: CUDA device, sm_90a, native library, one wgmma GEMM vs PyTorch
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 tools/run_check.py   # + NCCL all-reduce, P2P access, peer-memory barrier
 """
 import os
@@ -30,17 +30,17 @@ def main():
     torch.cuda.set_device(local)
     cap = torch.cuda.get_device_capability()
     props = torch.cuda.get_device_properties(local)
-    say(f"device {local}: {props.name}, sm_{cap[0]}{cap[1]}, {props.multi_processor_count} SMs, {props.total_memory / 2**30:.0f} GiB", cap == (10, 0))
+    say(f"device {local}: {props.name}, sm_{cap[0]}{cap[1]}, {props.multi_processor_count} SMs, {props.total_memory / 2**30:.0f} GiB", cap == (9, 0))
     from paddlefleetx_b200.ops import _native
 
     lib = _native.load()
     say(f"native kernel library loaded: {getattr(lib, '__file__', lib)}", lib is not None)
-    if lib is not None and cap == (10, 0):
+    if lib is not None and cap == (9, 0):
         a = torch.randn(512, 256, device="cuda").bfloat16()
         b = torch.randn(384, 256, device="cuda").bfloat16()
         y = lib.gemm(a, b, None, None, True, True, 0, 0, 0)
         err = float((y.float() - a.float() @ b.float().t()).norm() / (a.float() @ b.float().t()).norm())
-        say(f"tcgen05 GEMM vs fp32 reference: rel. error {err:.2e}", err < 1e-2)
+        say(f"wgmma GEMM vs fp32 reference: rel. error {err:.2e}", err < 1e-2)
     if world > 1:
         import torch.distributed as dist
 
