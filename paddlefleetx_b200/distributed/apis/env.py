@@ -73,6 +73,15 @@ def init_process_group(device: str = "gpu", timeout_s: int = 1800) -> None:
                             timeout=datetime.timedelta(seconds=timeout_s), **kwargs)
 
 
+def destroy_process_group() -> None:
+    """End of a launcher-started job: every rank meets at a barrier, then the default group and all subgroups are destroyed, so the
+    communicator's threads are joined before the interpreter shuts down (left alive, they can abort the process at exit).  No-op without
+    a process group."""
+    if dist.is_initialized():
+        dist.barrier()
+        dist.destroy_process_group()
+
+
 def set_hcg(hcg) -> None:
     global _hcg
     _hcg = hcg

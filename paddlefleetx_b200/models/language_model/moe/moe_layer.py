@@ -127,7 +127,8 @@ class MoELayer(nn.Module):
             gate_idx = gate_idx.unsqueeze(1)
         plan = make_plan(disp, gate_idx, x.shape[0])
         layer_key = self._layer_key if (self.training and torch.is_grad_enabled()) else None
-        if self.grouped is not None and x.dtype == torch.bfloat16:
+        ge = self.grouped
+        if ge is not None and OF.tensor_core_dtype(x, ge.w1, ge.b1, ge.w2, ge.b2):
             # sync-free: dispatch -> tile table -> 2 grouped GEMMs -> combine, all sized by the fixed capacity; the host never reads a count
             from .fused_dispatch import ALIGN
             from .grouped_experts import grouped_ffn

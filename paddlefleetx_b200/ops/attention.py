@@ -1,13 +1,13 @@
 """Attention front-end.
 
 ``attention(q, k, v)`` takes ``[b, s, heads, d]`` tensors (views are fine: the slices of a packed QKV projection, sequence-major
-storage).  Path selection on CUDA / bf16:
+storage).  Path selection on CUDA / bf16 or fp16 (q, k and v of one dtype):
   * training and inference at head_dim 128 or 64: our wgmma flash kernels — ``csrc/attention_fwd_sm90.cu`` and
     ``csrc/attention_bwd_sm90.cu`` — with in-kernel causal masking and counter-hash dropout (the backward regenerates the mask; nothing is
     stored).  ``flash_attention_packed`` is the same pair for the ``[b, s, heads, 3, d]`` output of a fused QKV projection: it reads q / k / v
     in place and writes ONE packed gradient, so no split / cat copies surround the kernels,
   * single-query decode steps over the static KV cache use ``csrc/attention_decode.cu`` (see models/.../gpt/model.py),
-  * explicit masks, other head sizes (backward), fp16 and CPU tensors: PyTorch SDPA — a *library* call, reported as such by the launch
+  * explicit masks, other head sizes, mixed dtypes, fp32 and CPU tensors: PyTorch SDPA — a *library* call, reported as such by the launch
     accounting (it does not count towards ``gpu_launches``); ``PFX_NATIVE_ATTN=0`` forces it everywhere,
   * the unfused reference path (QK^T -> fused causal softmax -> PV) used when ``use_flash_attn=False`` — this mirrors reference
     ``core_attn`` (hybrid_model.py:303-346).
@@ -27,7 +27,9 @@ _MASK64 = (1 << 64) - 1
 
 
 def _native_ok(q, k, v, attn_mask, causal, needs_grad: bool) -> bool:
-    if not _NATIVE or attn_mask is not None or not q.is_cuda or q.dtype != torch.bfloat16 or k.dtype != q.dtype or v.dtype != q.dtype:
+    from .functional import tensor_core_dtype
+
+    if not _NATIVE or attn_mask is not None or not q.is_cuda or not tensor_core_dtype(q, k, v):
         return False
     d = q.shape[-1]
     if d not in (64, 128) or q.shape[1] < 1 or (causal and k.shape[1] < q.shape[1]):

@@ -1,4 +1,4 @@
-// Flash-attention backward on wgmma / TMA (sm_90a), bf16, head_dim 128 or 64, causal or full, optional dropout.
+// Flash-attention backward on wgmma / TMA (sm_90a), bf16 or fp16 (a template parameter), head_dim 128 or 64, causal or full, optional dropout.
 //
 // One CTA owns a tile of 64 keys of one (batch, head) and walks the 64-query tiles that attend to it.  The score tile is computed
 // TRANSPOSED (keys on the wgmma M rows, queries on the columns), so that its accumulator fragment is directly the A fragment of the
@@ -15,7 +15,7 @@
 // The same shared-memory tiles serve as K-major and MN-major operands (a 128-byte-swizzled [rows x 64] panel is both), so Q_i,
 // dO_i, K_j, V_j are loaded once by TMA straight from the framework layout ([B, S, H, D] views, packed QKV included).  dQ is accumulated
 // across key tiles in an fp32 workspace: each dQ tile goes registers -> shared memory and ONE TMA reduce-add (cp.reduce.async.bulk.tensor)
-// folds it into global memory; the workspace is converted to bf16 afterwards; lse (log2 units) and delta = rowsum(dO o O) come from a small
+// folds it into global memory; the workspace is converted to the inputs' type afterwards; lse (log2 units) and delta = rowsum(dO o O) come from a small
 // preprocessing kernel.
 //
 // Warp roles (160 threads): warp 4 TMA producer (K/V once, then a 3-stage ring of Q_i / dO_i / lse_i / delta_i), warps 0-3 one consumer
@@ -81,7 +81,7 @@ __device__ __forceinline__ void tma_tile(const CUtensorMap* m, bool swapped, uin
   if (swapped) tma_load_3d(m, bar, dst, col, b, s); else tma_load_3d(m, bar, dst, col, s, b);
 }
 
-template <int kHd>
+template <int kHd, bool kBf16>   // kBf16: bf16 operands and gradients, otherwise fp16
 __global__ void __launch_bounds__(kBwThreads, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v,
                      const __grid_constant__ CUtensorMap tmap_do, const __grid_constant__ CUtensorMap tmap_dq, const __grid_constant__ BwParams prm) {
@@ -166,12 +166,12 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
 #pragma unroll
       for (int kk = 0; kk < kHd / 16; ++kk) {
         const uint32_t o = (kk / 4) * 8192 + (kk % 4) * 32;
-        WgmmaSS<kQt, true, 0, 0>::mma(s, wgmma_desc(s_k + o, kDescK), wgmma_desc(sq + o, kDescK), kk != 0 ? 1u : 0u);
+        WgmmaSS<kQt, kBf16, 0, 0>::mma(s, wgmma_desc(s_k + o, kDescK), wgmma_desc(sq + o, kDescK), kk != 0 ? 1u : 0u);
       }
 #pragma unroll
       for (int kk = 0; kk < kHd / 16; ++kk) {
         const uint32_t o = (kk / 4) * 8192 + (kk % 4) * 32;
-        WgmmaSS<kQt, true, 0, 0>::mma(dp, wgmma_desc(s_v + o, kDescK), wgmma_desc(sdo + o, kDescK), kk != 0 ? 1u : 0u);
+        WgmmaSS<kQt, kBf16, 0, 0>::mma(dp, wgmma_desc(s_v + o, kDescK), wgmma_desc(sdo + o, kDescK), kk != 0 ? 1u : 0u);
       }
       wgmma_commit();
       wgmma_wait<0>();
@@ -179,7 +179,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
       const float* dl_s = lse_s + kQt;
       // masks are decided per tile (warp-uniform branches): only diagonal / ragged tiles pay per-element compares
       const bool tile_mask = (prm.causal && (k0 + kKv - 1 > q0 + off)) || (k0 + kKv > prm.Sk);
-      uint32_t pw[kQt / 4], dsw[kQt / 4];                             // P_drop^T and dS^T as packed bf16 pairs, in wgmma A-fragment order
+      uint32_t pw[kQt / 4], dsw[kQt / 4];                             // P_drop^T and dS^T as packed 16-bit pairs, in wgmma A-fragment order
 #pragma unroll
       for (int g = 0; g < kQt / 8; ++g) {
         const int qc = 8 * g + col_in8;
@@ -202,11 +202,11 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
             if (!keep0) pd0 = 0.f;
             if (!keep1) pd1 = 0.f;
           }
-          pw[2 * g + hh] = pack_bf16x2(pd0, pd1);
-          dsw[2 * g + hh] = pack_bf16x2(p0 * (d0 - dl.x), p1 * (d1 - dl.y));                 // dS^T * scale = (P scale) o (drop(dP) - delta)
+          pw[2 * g + hh] = pack_16x2<kBf16>(pd0, pd1);
+          dsw[2 * g + hh] = pack_16x2<kBf16>(p0 * (d0 - dl.x), p1 * (d1 - dl.y));                 // dS^T * scale = (P scale) o (drop(dP) - delta)
         }
       }
-      // dS^T -> shared memory ([64 k x 64 q] bf16 panel, 128-byte swizzle) for the dQ product; the previous tile's dQ product has retired
+      // dS^T -> shared memory ([64 k x 64 q] 16-bit panel, 128-byte swizzle) for the dQ product; the previous tile's dQ product has retired
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         const uint32_t r = (uint32_t)(k_row + 8 * hh);
@@ -223,16 +223,16 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
 #pragma unroll
       for (int kk = 0; kk < kQt / 16; ++kk) {
         const uint32_t a[4] = {pw[4 * kk], pw[4 * kk + 1], pw[4 * kk + 2], pw[4 * kk + 3]};
-        WgmmaRS<kHd, 1>::mma(dv, a, wgmma_desc(sdo + kk * 2048, kDescMN), 1u);
+        WgmmaRS<kHd, 1, kBf16>::mma(dv, a, wgmma_desc(sdo + kk * 2048, kDescMN), 1u);
       }
 #pragma unroll
       for (int kk = 0; kk < kQt / 16; ++kk) {
         const uint32_t a[4] = {dsw[4 * kk], dsw[4 * kk + 1], dsw[4 * kk + 2], dsw[4 * kk + 3]};
-        WgmmaRS<kHd, 1>::mma(dk, a, wgmma_desc(sq + kk * 2048, kDescMN), 1u);
+        WgmmaRS<kHd, 1, kBf16>::mma(dk, a, wgmma_desc(sq + kk * 2048, kDescMN), 1u);
       }
 #pragma unroll
       for (int kk = 0; kk < kKv / 16; ++kk)
-        WgmmaSS<kHd, true, 1, 1>::mma(dq, wgmma_desc(s_ds + kk * 2048, kDescMN), wgmma_desc(s_k + kk * 2048, kDescMN), kk != 0 ? 1u : 0u);
+        WgmmaSS<kHd, kBf16, 1, 1>::mma(dq, wgmma_desc(s_ds + kk * 2048, kDescMN), wgmma_desc(s_k + kk * 2048, kDescMN), kk != 0 ? 1u : 0u);
       wgmma_commit();
       wgmma_wait<0>();
       if (lane == 0) mbar_arrive(q_empty(st));
@@ -258,12 +258,12 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
     for (int hh = 0; hh < 2; ++hh) {
       const int kg = k0 + k_row + 8 * hh;
       if (kg < prm.Sk) {
-        __nv_bfloat16* pv = reinterpret_cast<__nv_bfloat16*>(prm.dv.ptr) + (size_t)b * prm.dv.sb + (size_t)kg * prm.dv.ss + (size_t)h * prm.dv.sh + col_in8;
-        __nv_bfloat16* pk = reinterpret_cast<__nv_bfloat16*>(prm.dk.ptr) + (size_t)b * prm.dk.sb + (size_t)kg * prm.dk.ss + (size_t)h * prm.dk.sh + col_in8;
+        uint16_t* pv = reinterpret_cast<uint16_t*>(prm.dv.ptr) + (size_t)b * prm.dv.sb + (size_t)kg * prm.dv.ss + (size_t)h * prm.dv.sh + col_in8;
+        uint16_t* pk = reinterpret_cast<uint16_t*>(prm.dk.ptr) + (size_t)b * prm.dk.sb + (size_t)kg * prm.dk.ss + (size_t)h * prm.dk.sh + col_in8;
 #pragma unroll
         for (int g = 0; g < kHd / 8; ++g) {
-          *reinterpret_cast<uint32_t*>(pv + 8 * g) = pack_bf16x2(dv[4 * g + 2 * hh], dv[4 * g + 2 * hh + 1]);
-          *reinterpret_cast<uint32_t*>(pk + 8 * g) = pack_bf16x2(dk[4 * g + 2 * hh], dk[4 * g + 2 * hh + 1]);
+          *reinterpret_cast<uint32_t*>(pv + 8 * g) = pack_16x2<kBf16>(dv[4 * g + 2 * hh], dv[4 * g + 2 * hh + 1]);
+          *reinterpret_cast<uint32_t*>(pk + 8 * g) = pack_16x2<kBf16>(dk[4 * g + 2 * hh], dk[4 * g + 2 * hh + 1]);
         }
       }
     }
@@ -271,8 +271,8 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
 }
 
 // ---- preprocessing: delta = rowsum(dO o O), lse in log2 units; both padded to a multiple of 64 queries per (b, h)
-template <int kHd>
-__global__ void attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, int64_t o_sb, int64_t o_ss, int64_t o_sh, const __nv_bfloat16* __restrict__ dout,
+template <int kHd, bool kBf16>
+__global__ void attn_bwd_prep_kernel(const uint16_t* __restrict__ o, int64_t o_sb, int64_t o_ss, int64_t o_sh, const uint16_t* __restrict__ dout,
                                      int64_t d_sb, int64_t d_ss, int64_t d_sh, const float* __restrict__ lse, float* __restrict__ lse2,
                                      float* __restrict__ delta, int B, int Sq, int H, int Sq_pad) {
   const int64_t w = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);      // (b, s_pad, h)
@@ -287,12 +287,12 @@ __global__ void attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, int64_
     return;
   }
   constexpr int kPer = kHd / 32;                         // channels per lane (4 or 2)
-  const __nv_bfloat162* a2 = reinterpret_cast<const __nv_bfloat162*>(o + b * o_sb + s * o_ss + h * o_sh + lane * kPer);
-  const __nv_bfloat162* g2 = reinterpret_cast<const __nv_bfloat162*>(dout + b * d_sb + s * d_ss + h * d_sh + lane * kPer);
+  const uint16_t* a2 = o + b * o_sb + s * o_ss + h * o_sh + lane * kPer;
+  const uint16_t* g2 = dout + b * d_sb + s * d_ss + h * d_sh + lane * kPer;
   float acc = 0.f;
 #pragma unroll
   for (int i = 0; i < kPer / 2; ++i) {
-    const float2 x = __bfloat1622float2(a2[i]), y = __bfloat1622float2(g2[i]);
+    const float2 x = load_16x2<kBf16>(a2 + 2 * i), y = load_16x2<kBf16>(g2 + 2 * i);
     acc += x.x * y.x + x.y * y.y;
   }
   acc = warp_sum(acc);
@@ -302,8 +302,9 @@ __global__ void attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, int64_
   }
 }
 
-// ---- dq: fp32 accumulator -> bf16 view
-__global__ void attn_bwd_dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict__ dq, int64_t sb, int64_t ss, int64_t sh, int B, int Sq, int H, int kHd) {
+// ---- dq: fp32 accumulator -> 16-bit view
+template <bool kBf16>
+__global__ void attn_bwd_dq_convert_kernel(const float* __restrict__ acc, uint16_t* __restrict__ dq, int64_t sb, int64_t ss, int64_t sh, int B, int Sq, int H, int kHd) {
   const int64_t n8 = (int64_t)B * Sq * H * (kHd / 8);
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += (int64_t)gridDim.x * blockDim.x) {
     const int c = (int)(i % (kHd / 8));
@@ -313,7 +314,7 @@ __global__ void attn_bwd_dq_convert_kernel(const float* __restrict__ acc, __nv_b
     const int b = (int)(row / ((int64_t)H * Sq));
     const float4 x = *reinterpret_cast<const float4*>(acc + i * 8), y = *reinterpret_cast<const float4*>(acc + i * 8 + 4);
     uint4 v;
-    v.x = pack_bf16x2(x.x, x.y); v.y = pack_bf16x2(x.z, x.w); v.z = pack_bf16x2(y.x, y.y); v.w = pack_bf16x2(y.z, y.w);
+    v.x = pack_16x2<kBf16>(x.x, x.y); v.y = pack_16x2<kBf16>(x.z, x.w); v.z = pack_16x2<kBf16>(y.x, y.y); v.w = pack_16x2<kBf16>(y.z, y.w);
     *reinterpret_cast<uint4*>(dq + b * sb + s * ss + h * sh + c * 8) = v;
   }
 }
@@ -322,18 +323,19 @@ bool view_ok(const AttnView& t) {
   return t.ptr != nullptr && (reinterpret_cast<uintptr_t>(t.ptr) % 16) == 0 && t.sb % 8 == 0 && t.ss % 8 == 0 && t.sh % 8 == 0;
 }
 
-bool make_map(CUtensorMap* m, const AttnView& t, int B, int S, int H, int D, uint32_t box_rows, bool* swapped) {
+bool make_map(CUtensorMap* m, const AttnView& t, int dtype, int B, int S, int H, int D, uint32_t box_rows, bool* swapped) {
   const uint64_t inner = (uint64_t)(H - 1) * t.sh + D;
-  return make_tmap_bshd(m, t.ptr, 1, inner, (uint64_t)S, (uint64_t)B, (uint64_t)t.ss * 2, (uint64_t)t.sb * 2, 64, box_rows, swapped);
+  return make_tmap_bshd(m, t.ptr, dtype, inner, (uint64_t)S, (uint64_t)B, (uint64_t)t.ss * 2, (uint64_t)t.sb * 2, 64, box_rows, swapped);
 }
 
 }  // namespace
 
-template <int kHd>
+template <int kHd, bool kBf16>
 static cudaError_t attention_bwd_impl(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, const AttnView& dout, const float* lse,
                                       const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int Sq,
                                       int Sk, int H, float scale, bool causal, AttnDropout drop, cudaStream_t st) {
   constexpr int D = kHd;
+  constexpr int dt = kBf16 ? 1 : 0;
   using S = BwSmem<kHd>;
   const int Sq_pad = (Sq + kQt - 1) / kQt * kQt;
   cudaError_t e = cudaMemsetAsync(dq_acc, 0, (size_t)B * Sq * H * kHd * sizeof(float), st);
@@ -341,14 +343,14 @@ static cudaError_t attention_bwd_impl(const AttnView& q, const AttnView& k, cons
   {
     const int64_t warps = (int64_t)B * Sq_pad * H;
     const int wpb = 8;
-    attn_bwd_prep_kernel<kHd><<<(unsigned)((warps + wpb - 1) / wpb), wpb * 32, 0, st>>>(
-        (const __nv_bfloat16*)out.ptr, out.sb, out.ss, out.sh, (const __nv_bfloat16*)dout.ptr, dout.sb, dout.ss, dout.sh, lse, lse2, delta, B, Sq, H, Sq_pad);
+    attn_bwd_prep_kernel<kHd, kBf16><<<(unsigned)((warps + wpb - 1) / wpb), wpb * 32, 0, st>>>(
+        (const uint16_t*)out.ptr, out.sb, out.ss, out.sh, (const uint16_t*)dout.ptr, dout.sb, dout.ss, dout.sh, lse, lse2, delta, B, Sq, H, Sq_pad);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
   }
   CUtensorMap tq, tk, tv, tdo, tdq;
   bool sq = false, sk = false, sv = false, sdo = false;
-  bool ok = make_map(&tq, q, B, Sq, H, D, kQt, &sq) && make_map(&tk, k, B, Sk, H, D, kKv, &sk) && make_map(&tv, v, B, Sk, H, D, kKv, &sv) &&
-            make_map(&tdo, dout, B, Sq, H, D, kQt, &sdo) &&
+  bool ok = make_map(&tq, q, dt, B, Sq, H, D, kQt, &sq) && make_map(&tk, k, dt, B, Sk, H, D, kKv, &sk) && make_map(&tv, v, dt, B, Sk, H, D, kKv, &sv) &&
+            make_map(&tdo, dout, dt, B, Sq, H, D, kQt, &sdo) &&
             make_tmap_2d_plain(&tdq, dq_acc, 3, (uint64_t)H * kHd, (uint64_t)B * Sq, (uint64_t)H * kHd * 4, kHd, kQt);
   if (!ok) return cudaErrorInvalidValue;
   BwParams prm{};
@@ -365,23 +367,27 @@ static cudaError_t attention_bwd_impl(const AttnView& q, const AttnView& k, cons
   prm.seed = drop.seed;
   static bool attr_set = false;
   if (!attr_set) {
-    if ((e = cudaFuncSetAttribute(attention_bwd_kernel<kHd>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(attention_bwd_kernel<kHd, kBf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal)) != cudaSuccess) return e;
     attr_set = true;
   }
   const int n_kv = (Sk + kKv - 1) / kKv;
-  attention_bwd_kernel<kHd><<<(unsigned)(n_kv * B * H), kBwThreads, S::kTotal, st>>>(tq, tk, tv, tdo, tdq, prm);
+  attention_bwd_kernel<kHd, kBf16><<<(unsigned)(n_kv * B * H), kBwThreads, S::kTotal, st>>>(tq, tk, tv, tdo, tdq, prm);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  attn_bwd_dq_convert_kernel<<<1184, 256, 0, st>>>(dq_acc, (__nv_bfloat16*)const_cast<void*>(dq.ptr), dq.sb, dq.ss, dq.sh, B, Sq, H, kHd);
+  attn_bwd_dq_convert_kernel<kBf16><<<1184, 256, 0, st>>>(dq_acc, (uint16_t*)const_cast<void*>(dq.ptr), dq.sb, dq.ss, dq.sh, B, Sq, H, kHd);
   return cudaGetLastError();
 }
 
 cudaError_t attention_bwd(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, const AttnView& dout, const float* lse,
                           const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int Sq,
-                          int Sk, int H, int D, float scale, bool causal, AttnDropout drop, cudaStream_t st) {
-  if ((D != 64 && D != 128) || B < 1 || Sq < 1 || Sk < 1 || (causal && Sk < Sq)) return cudaErrorInvalidValue;
+                          int Sk, int H, int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st) {
+  if ((D != 64 && D != 128) || (dtype != 0 && dtype != 1) || B < 1 || Sq < 1 || Sk < 1 || (causal && Sk < Sq)) return cudaErrorInvalidValue;
   for (const AttnView* t : {&q, &k, &v, &out, &dout, &dq, &dk, &dv}) if (!view_ok(*t)) return cudaErrorInvalidValue;
-  if (D == 128) return attention_bwd_impl<128>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, Sq, Sk, H, scale, causal, drop, st);
-  return attention_bwd_impl<64>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, Sq, Sk, H, scale, causal, drop, st);
+  if (dtype == 1) {
+    if (D == 128) return attention_bwd_impl<128, true>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, Sq, Sk, H, scale, causal, drop, st);
+    return attention_bwd_impl<64, true>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, Sq, Sk, H, scale, causal, drop, st);
+  }
+  if (D == 128) return attention_bwd_impl<128, false>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, Sq, Sk, H, scale, causal, drop, st);
+  return attention_bwd_impl<64, false>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, Sq, Sk, H, scale, causal, drop, st);
 }
 
 }  // namespace pfx

@@ -1,4 +1,4 @@
-// Flash-style attention forward on wgmma / TMA (sm_90a), bf16, head_dim 64 or 128, causal or full, optional dropout.
+// Flash-style attention forward on wgmma / TMA (sm_90a), bf16 or fp16 (a template parameter), head_dim 64 or 128, causal or full, optional dropout.
 //
 //   O[b, s, h, :] = softmax(scale * Q[b, s, h, :] . K[b, :, h, :]^T (+ causal mask)) (dropout) @ V[b, :, h, :]
 //
@@ -14,7 +14,7 @@
 //             as the MN-major B operand; O accumulates in registers.
 // Shared memory per CTA is 72 KB (D = 64) or 144 KB (D = 128); registers allow two CTAs per SM at D = 64 and one at D = 128 (the launcher
 // asks the occupancy calculator and sizes the persistent grid to what is resident).
-// Causal tiles above the diagonal are never loaded; masks are applied only on diagonal / ragged tiles.  Output O (bf16) and the row-wise
+// Causal tiles above the diagonal are never loaded; masks are applied only on diagonal / ragged tiles.  Output O (the inputs' type) and the row-wise
 // log-sum-exp (fp32, [B, H, S]) are written from registers.  Reference call site: flash_attention in hybrid_model.py:284-301
 // (FlashAttention-2 library on Ampere mma.sync).
 #include <cstdio>
@@ -52,10 +52,10 @@ __device__ __forceinline__ void tma3(const CUtensorMap* m, bool swapped, uint32_
   if (swapped) tma_load_3d(m, bar, dst, col, b, s); else tma_load_3d(m, bar, dst, col, s, b);
 }
 
-template <int kD, bool kCausal>
+template <int kD, bool kCausal, bool kBf16>   // kBf16: bf16 operands and output, otherwise fp16
 __global__ void __launch_bounds__(kFaThreads, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v,
-                     __nv_bfloat16* __restrict__ out, int64_t o_sb, int64_t o_ss, int64_t o_sh, float* __restrict__ lse, int B, int Sq, int Sk, int H,
+                     uint16_t* __restrict__ out, int64_t o_sb, int64_t o_ss, int64_t o_sh, float* __restrict__ lse, int B, int Sq, int Sk, int H,
                      float scale_log2, int hs_q, int hs_k, int hs_v, uint32_t swapped, uint32_t drop_thresh16, float inv_keep, uint64_t seed) {
   using S = FaSmem<kD>;
   constexpr int kPanels = kD / 64;                 // 64-element (128-byte) column panels of a D-wide tile
@@ -139,7 +139,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
 #pragma unroll
         for (int k = 0; k < kD / 16; ++k) {
           const uint32_t offq = (k / 4) * (kFaQ * 128) + (k % 4) * 32, offk = (k / 4) * (kFaKv * 128) + (k % 4) * 32;
-          WgmmaSS<kFaKv, true, 0, 0>::mma(s, wgmma_desc(smem_q + offq, kDescK), wgmma_desc(sk + offk, kDescK), k != 0 ? 1u : 0u);
+          WgmmaSS<kFaKv, kBf16, 0, 0>::mma(s, wgmma_desc(smem_q + offq, kDescK), wgmma_desc(sk + offk, kDescK), k != 0 ? 1u : 0u);
         }
         wgmma_commit();
         wgmma_wait<0>();
@@ -169,7 +169,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
         }
 #pragma unroll
         for (int i = 0; i < kD / 2; ++i) o[i] *= f[(i >> 1) & 1];
-        uint32_t pw[kFaKv / 4];                    // the probabilities as packed bf16 pairs, in wgmma A-fragment order
+        uint32_t pw[kFaKv / 4];                    // the probabilities as packed 16-bit pairs, in wgmma A-fragment order
 #pragma unroll
         for (int g = 0; g < kFaKv / 8; ++g) {
 #pragma unroll
@@ -183,7 +183,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
               if ((bits & 0xFFFFu) < drop_thresh16) p0 = 0.f;
               if ((bits >> 16) < drop_thresh16) p1 = 0.f;
             }
-            pw[2 * g + hh] = pack_bf16x2(p0, p1);
+            pw[2 * g + hh] = pack_16x2<kBf16>(p0, p1);
           }
         }
         wgmma_fence();
@@ -191,7 +191,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
         for (int k = 0; k < kFaKv / 16; ++k) {
           const uint32_t b_off = (k / 4) * (kPanels * 8192) + (k % 4) * 2048;              // V: 64-key blocks, 16 keys = 2 KB
           const uint32_t a[4] = {pw[4 * k], pw[4 * k + 1], pw[4 * k + 2], pw[4 * k + 3]};
-          WgmmaRS<kD, 1>::mma(o, a, wgmma_desc(sv + b_off, kDescMN), 1u);
+          WgmmaRS<kD, 1, kBf16>::mma(o, a, wgmma_desc(sv + b_off, kDescMN), 1u);
         }
         wgmma_commit();
         wgmma_wait<0>();
@@ -207,10 +207,10 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
         const int row_g = q0 + row_lo + 8 * hh;
         const float inv = l_all > 0.f ? inv_keep / l_all : 0.f;
         if (row_g < Sq) {
-          __nv_bfloat16* dst = out + (size_t)b * o_sb + (size_t)row_g * o_ss + (size_t)h * o_sh + col_in8;
+          uint16_t* dst = out + (size_t)b * o_sb + (size_t)row_g * o_ss + (size_t)h * o_sh + col_in8;
 #pragma unroll
           for (int g = 0; g < kD / 8; ++g)
-            *reinterpret_cast<uint32_t*>(dst + 8 * g) = pack_bf16x2(o[4 * g + 2 * hh] * inv, o[4 * g + 2 * hh + 1] * inv);
+            *reinterpret_cast<uint32_t*>(dst + 8 * g) = pack_16x2<kBf16>(o[4 * g + 2 * hh] * inv, o[4 * g + 2 * hh + 1] * inv);
           if (lse != nullptr && (lane & 3u) == 0)
             lse[((size_t)b * H + h) * Sq + row_g] = (l_all > 0.f) ? (m_run[hh] + log2f(l_all)) * 0.6931471805599453f : -INFINITY;
         }
@@ -219,18 +219,19 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
   }
 }
 
-template <int kD, bool kCausal>
+template <int kD, bool kCausal, bool kBf16>
 cudaError_t launch_fa(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H, float scale,
                       AttnDropout drop, cudaStream_t st) {
   using S = FaSmem<kD>;
   CUtensorMap tq, tk, tv;
   bool sq = false, sk = false, sv = false;
   auto inner = [&](const AttnView& t) { return (uint64_t)(H - 1) * t.sh + kD; };
-  bool ok = make_tmap_bshd(&tq, q.ptr, 1, inner(q), Sq, B, (uint64_t)q.ss * 2, (uint64_t)q.sb * 2, 64, kFaQ, &sq);
-  ok &= make_tmap_bshd(&tk, k.ptr, 1, inner(k), Sk, B, (uint64_t)k.ss * 2, (uint64_t)k.sb * 2, 64, kFaKv, &sk);
-  ok &= make_tmap_bshd(&tv, v.ptr, 1, inner(v), Sk, B, (uint64_t)v.ss * 2, (uint64_t)v.sb * 2, 64, 64, &sv);
+  constexpr int dt = kBf16 ? 1 : 0;
+  bool ok = make_tmap_bshd(&tq, q.ptr, dt, inner(q), Sq, B, (uint64_t)q.ss * 2, (uint64_t)q.sb * 2, 64, kFaQ, &sq);
+  ok &= make_tmap_bshd(&tk, k.ptr, dt, inner(k), Sk, B, (uint64_t)k.ss * 2, (uint64_t)k.sb * 2, 64, kFaKv, &sk);
+  ok &= make_tmap_bshd(&tv, v.ptr, dt, inner(v), Sk, B, (uint64_t)v.ss * 2, (uint64_t)v.sb * 2, 64, 64, &sv);
   if (!ok) return cudaErrorInvalidValue;
-  auto kern = attention_fwd_kernel<kD, kCausal>;
+  auto kern = attention_fwd_kernel<kD, kCausal, kBf16>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal);
@@ -247,27 +248,34 @@ cudaError_t launch_fa(const AttnView& q, const AttnView& k, const AttnView& v, c
   const uint32_t thresh = drop.p > 0.f ? (uint32_t)(drop.p * 65536.f + 0.5f) : 0u;
   const float inv_keep = drop.p > 0.f ? 1.f / (1.f - drop.p) : 1.f;
   const uint32_t swapped = (sq ? 1u : 0u) | (sk ? 2u : 0u) | (sv ? 4u : 0u);
-  kern<<<grid, kFaThreads, S::kTotal, st>>>(tq, tk, tv, (__nv_bfloat16*)const_cast<void*>(out.ptr), out.sb, out.ss, out.sh, lse, B, Sq, Sk, H,
+  kern<<<grid, kFaThreads, S::kTotal, st>>>(tq, tk, tv, (uint16_t*)const_cast<void*>(out.ptr), out.sb, out.ss, out.sh, lse, B, Sq, Sk, H,
                                             scale * 1.4426950408889634f, (int)q.sh, (int)k.sh, (int)v.sh, swapped, thresh, inv_keep, drop.seed);
   return cudaGetLastError();
+}
+
+template <bool kBf16>
+cudaError_t launch_fa_dt(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H,
+                         int D, float scale, bool causal, AttnDropout drop, cudaStream_t st) {
+  if (D == 128) return causal ? launch_fa<128, true, kBf16>(q, k, v, out, lse, B, Sq, Sk, H, scale, drop, st) : launch_fa<128, false, kBf16>(q, k, v, out, lse, B, Sq, Sk, H, scale, drop, st);
+  return causal ? launch_fa<64, true, kBf16>(q, k, v, out, lse, B, Sq, Sk, H, scale, drop, st) : launch_fa<64, false, kBf16>(q, k, v, out, lse, B, Sq, Sk, H, scale, drop, st);
 }
 
 }  // namespace
 
 cudaError_t attention_fwd_v2(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H,
-                             int D, float scale, bool causal, AttnDropout drop, cudaStream_t st) {
-  if ((D != 64 && D != 128) || B < 1 || Sq < 1 || Sk < 1 || (causal && Sk < Sq)) return cudaErrorInvalidValue;
+                             int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st) {
+  if ((D != 64 && D != 128) || (dtype != 0 && dtype != 1) || B < 1 || Sq < 1 || Sk < 1 || (causal && Sk < Sq)) return cudaErrorInvalidValue;
   for (const AttnView* t : {&q, &k, &v, &out})
     if (t->ptr == nullptr || (reinterpret_cast<uintptr_t>(t->ptr) % 16) || t->sb % 8 || t->ss % 8 || t->sh % 8) return cudaErrorInvalidValue;
-  if (D == 128) return causal ? launch_fa<128, true>(q, k, v, out, lse, B, Sq, Sk, H, scale, drop, st) : launch_fa<128, false>(q, k, v, out, lse, B, Sq, Sk, H, scale, drop, st);
-  return causal ? launch_fa<64, true>(q, k, v, out, lse, B, Sq, Sk, H, scale, drop, st) : launch_fa<64, false>(q, k, v, out, lse, B, Sq, Sk, H, scale, drop, st);
+  return dtype == 1 ? launch_fa_dt<true>(q, k, v, out, lse, B, Sq, Sk, H, D, scale, causal, drop, st)
+                    : launch_fa_dt<false>(q, k, v, out, lse, B, Sq, Sk, H, D, scale, causal, drop, st);
 }
 
 cudaError_t attention_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Sq, int Sk, int H, int D, float scale,
                           bool causal, cudaStream_t st) {
   const int64_t hd = (int64_t)H * D;
   const AttnView vq{q, (int64_t)Sq * hd, hd, D}, vk{k, (int64_t)Sk * hd, hd, D}, vv{v, (int64_t)Sk * hd, hd, D}, vo{out, (int64_t)Sq * hd, hd, D};
-  return attention_fwd_v2(vq, vk, vv, vo, lse, B, Sq, Sk, H, D, scale, causal, AttnDropout{0.f, 0}, st);
+  return attention_fwd_v2(vq, vk, vv, vo, lse, B, Sq, Sk, H, D, scale, causal, AttnDropout{0.f, 0}, 1, st);
 }
 
 }  // namespace pfx

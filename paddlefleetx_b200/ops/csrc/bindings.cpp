@@ -21,6 +21,7 @@ inline int dtype_code(const at::Tensor& t) {
     default: TORCH_CHECK(false, "pfx: unsupported dtype ", t.scalar_type());
   }
 }
+inline bool is_16bit(const at::Tensor& t) { return t.scalar_type() == at::kBFloat16 || t.scalar_type() == at::kHalf; }
 inline cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
 inline int num_sms() {
   static int n = 0;
@@ -68,7 +69,8 @@ at::Tensor gemm(const at::Tensor& a, const at::Tensor& b, c10::optional<at::Tens
   g.a = a.data_ptr(); g.b = b.data_ptr(); g.d = d.data_ptr();
   g.bias = nullptr;
   if (bias.has_value() && bias->defined()) {
-    TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->numel() == N && bias->is_contiguous(), "gemm: bias must be bf16 [N]");
+    TORCH_CHECK(bias->scalar_type() == a.scalar_type() && bias->numel() == N && bias->is_contiguous(), "gemm: bias must be [N] of the operands' dtype (",
+                a.scalar_type(), "), got ", bias->scalar_type());
     TORCH_CHECK(N % 8 == 0, "gemm: bias epilogue needs N % 8 == 0");
     g.bias = bias->data_ptr();
   } else {
@@ -87,8 +89,8 @@ at::Tensor gemm(const at::Tensor& a, const at::Tensor& b, c10::optional<at::Tens
 // FFN1 forward in one kernel: z = x W^T + b (kept for the backward) and g = gelu(z), both written by the GEMM epilogue.
 std::vector<at::Tensor> gemm_bias_gelu_dual(const at::Tensor& x, const at::Tensor& w, const at::Tensor& bias) {
   TORCH_CHECK(x.is_cuda() && x.dim() == 2 && w.dim() == 2 && x.is_contiguous() && w.is_contiguous() && x.size(1) == w.size(1), "gemm_bias_gelu_dual: x [M,K], w [N,K]");
-  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && bias.scalar_type() == at::kBFloat16 && bias.numel() == w.size(0) &&
-              bias.is_contiguous(), "gemm_bias_gelu_dual: bf16 operands, bias [N]");
+  TORCH_CHECK(is_16bit(x) && w.scalar_type() == x.scalar_type() && bias.scalar_type() == x.scalar_type() && bias.numel() == w.size(0) &&
+              bias.is_contiguous(), "gemm_bias_gelu_dual: bf16 or fp16 operands of one dtype, bias [N]");
   TORCH_CHECK(w.size(0) % 8 == 0 && x.size(1) % 8 == 0, "gemm_bias_gelu_dual: N, K multiples of 8");
   const c10::cuda::CUDAGuard guard(x.device());
   at::Tensor z = at::empty({x.size(0), w.size(0)}, x.options()), gl = at::empty({x.size(0), w.size(0)}, x.options());
@@ -96,7 +98,7 @@ std::vector<at::Tensor> gemm_bias_gelu_dual(const at::Tensor& x, const at::Tenso
   g.a = x.data_ptr(); g.b = w.data_ptr(); g.d = z.data_ptr(); g.d2 = gl.data_ptr(); g.bias = bias.data_ptr();
   g.M = (int)x.size(0); g.N = (int)w.size(0); g.K = (int)x.size(1);
   g.lda = (int)x.stride(0); g.ldb = (int)w.stride(0); g.ldd = (int)z.stride(0);
-  g.a_kmajor = true; g.b_kmajor = true; g.out_mode = 0; g.epilogue = pfx::EPI_BIAS_GELU_DUAL; g.ab_format = 1; g.num_sms = num_sms(); g.config = 0;
+  g.a_kmajor = true; g.b_kmajor = true; g.out_mode = 0; g.epilogue = pfx::EPI_BIAS_GELU_DUAL; g.ab_format = dtype_code(x); g.num_sms = num_sms(); g.config = 0;
   PFX_CUDA_CHECK(pfx::gemm_wgmma(g, cur_stream()));
   return {z, gl};
 }
@@ -105,7 +107,7 @@ std::vector<at::Tensor> gemm_bias_gelu_dual(const at::Tensor& x, const at::Tenso
 at::Tensor gemm_dgelu(const at::Tensor& dy, const at::Tensor& w, const at::Tensor& z) {
   TORCH_CHECK(dy.is_cuda() && dy.dim() == 2 && w.dim() == 2 && z.dim() == 2 && dy.is_contiguous() && w.is_contiguous() && z.is_contiguous(), "gemm_dgelu: contiguous 2-D");
   TORCH_CHECK(dy.size(1) == w.size(0) && z.size(0) == dy.size(0) && z.size(1) == w.size(1), "gemm_dgelu: dy [M,K], w [K,N], z [M,N]");
-  TORCH_CHECK(dy.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && z.scalar_type() == at::kBFloat16, "gemm_dgelu: bf16 only");
+  TORCH_CHECK(is_16bit(dy) && w.scalar_type() == dy.scalar_type() && z.scalar_type() == dy.scalar_type(), "gemm_dgelu: bf16 or fp16 operands of one dtype");
   TORCH_CHECK(w.size(1) % 8 == 0 && w.size(0) % 8 == 0, "gemm_dgelu: N, K multiples of 8");
   const c10::cuda::CUDAGuard guard(dy.device());
   at::Tensor dz = at::empty_like(z);
@@ -113,7 +115,7 @@ at::Tensor gemm_dgelu(const at::Tensor& dy, const at::Tensor& w, const at::Tenso
   g.a = dy.data_ptr(); g.b = w.data_ptr(); g.d = dz.data_ptr(); g.aux = z.data_ptr(); g.ld_aux = (int)z.stride(0);
   g.M = (int)dy.size(0); g.N = (int)w.size(1); g.K = (int)dy.size(1);
   g.lda = (int)dy.stride(0); g.ldb = (int)w.stride(0); g.ldd = (int)dz.stride(0);
-  g.a_kmajor = true; g.b_kmajor = false; g.out_mode = 0; g.epilogue = pfx::EPI_DGELU; g.ab_format = 1; g.num_sms = num_sms(); g.config = 0;
+  g.a_kmajor = true; g.b_kmajor = false; g.out_mode = 0; g.epilogue = pfx::EPI_DGELU; g.ab_format = dtype_code(dy); g.num_sms = num_sms(); g.config = 0;
   PFX_CUDA_CHECK(pfx::gemm_wgmma(g, cur_stream()));
   return dz;
 }
@@ -617,10 +619,12 @@ at::Tensor gemv_w8a8(const at::Tensor& xq, const at::Tensor& wq, const at::Tenso
 
 at::Tensor gemm_smallm(const at::Tensor& x, const at::Tensor& w, c10::optional<at::Tensor> bias, int64_t split) {
   TORCH_CHECK(x.is_cuda() && x.dim() == 2 && w.dim() == 2 && x.is_contiguous() && w.is_contiguous() && x.size(1) == w.size(1), "gemm_smallm: x [M,K], w [N,K]");
-  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16, "gemm_smallm: bf16 only");
+  TORCH_CHECK(is_16bit(x) && w.scalar_type() == x.scalar_type(), "gemm_smallm: bf16 or fp16 operands of one dtype");
+  const bool has_bias = bias.has_value() && bias->defined();
+  if (has_bias) TORCH_CHECK(bias->scalar_type() == x.scalar_type() && bias->is_contiguous() && bias->numel() == w.size(0), "gemm_smallm: bias [N] of the operands' dtype");
   at::Tensor y = at::empty({x.size(0), w.size(0)}, x.options());
-  const void* b = (bias.has_value() && bias->defined()) ? bias->data_ptr() : nullptr;
-  PFX_CUDA_CHECK(pfx::gemm_smallm(x.data_ptr(), w.data_ptr(), b, y.data_ptr(), (int)x.size(0), (int)w.size(0), (int)x.size(1), 1, (int)split,
+  const void* b = has_bias ? bias->data_ptr() : nullptr;
+  PFX_CUDA_CHECK(pfx::gemm_smallm(x.data_ptr(), w.data_ptr(), b, y.data_ptr(), (int)x.size(0), (int)w.size(0), (int)x.size(1), dtype_code(x), (int)split,
                                   at::cuda::getCurrentDeviceProperties()->multiProcessorCount, cur_stream()));
   return y;
 }
@@ -690,32 +694,35 @@ void embedding_bwd_(const at::Tensor& ids, const at::Tensor& dout, at::Tensor& d
 }
 
 static pfx::AttnView attn_view(const at::Tensor& t, const char* name) {
-  TORCH_CHECK(t.is_cuda() && t.dim() == 4 && t.scalar_type() == at::kBFloat16 && t.stride(3) == 1, name, ": [B,S,H,D] bf16 CUDA view with contiguous D expected");
+  TORCH_CHECK(t.is_cuda() && t.dim() == 4 && is_16bit(t) && t.stride(3) == 1, name, ": [B,S,H,D] bf16 or fp16 CUDA view with contiguous D expected");
   TORCH_CHECK(t.stride(0) % 8 == 0 && t.stride(1) % 8 == 0 && t.stride(2) % 8 == 0 && (reinterpret_cast<uintptr_t>(t.data_ptr()) % 16) == 0,
               name, ": strides must be multiples of 8 elements and the base 16-byte aligned");
   return pfx::AttnView{t.data_ptr(), t.stride(0), t.stride(1), t.stride(2)};
 }
 
-// Flash attention forward on [B,S,H,D] bf16 views (no copies for packed-QKV slices / sequence-major storage); optional dropout keyed by `seed`.
+// Flash attention forward on [B,S,H,D] bf16 or fp16 views (no copies for packed-QKV slices / sequence-major storage); optional dropout keyed by `seed`.
 std::vector<at::Tensor> attention_fwd_v2(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v, bool causal, double scale, double dropout_p,
                                          int64_t seed) {
   TORCH_CHECK(q.dim() == 4 && k.dim() == 4 && k.sizes() == v.sizes() && q.size(0) == k.size(0) && q.size(2) == k.size(2) && q.size(3) == k.size(3),
               "attention_fwd_v2: shape mismatch");
+  TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type(), "attention_fwd_v2: q, k, v must have one dtype");
   const c10::cuda::CUDAGuard guard(q.device());
   auto out = at::empty({q.size(0), q.size(1), q.size(2), q.size(3)}, q.options());
   auto lse = at::empty({q.size(0), q.size(2), q.size(1)}, q.options().dtype(at::kFloat));
   PFX_CUDA_CHECK(pfx::attention_fwd_v2(attn_view(q, "q"), attn_view(k, "k"), attn_view(v, "v"), attn_view(out, "out"), lse.data_ptr<float>(),
                                        (int)q.size(0), (int)q.size(1), (int)k.size(1), (int)q.size(2), (int)q.size(3), (float)scale, causal,
-                                       pfx::AttnDropout{(float)dropout_p, (uint64_t)seed}, cur_stream()));
+                                       pfx::AttnDropout{(float)dropout_p, (uint64_t)seed}, dtype_code(q), cur_stream()));
   return {out, lse};
 }
 
-// Flash attention backward (head_dim 128): writes dq / dk / dv into the given (possibly strided) views.
+// Flash attention backward (head_dim 64 or 128, bf16 or fp16): writes dq / dk / dv into the given (possibly strided) views.
 void attention_bwd(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v, const at::Tensor& out, const at::Tensor& dout, const at::Tensor& lse,
                    at::Tensor& dq, at::Tensor& dk, at::Tensor& dv, bool causal, double scale, double dropout_p, int64_t seed) {
   TORCH_CHECK(q.dim() == 4 && k.sizes() == v.sizes() && q.sizes() == out.sizes() && q.sizes() == dout.sizes() && q.sizes() == dq.sizes() &&
               k.sizes() == dk.sizes() && k.sizes() == dv.sizes() && (q.size(3) == 128 || q.size(3) == 64), "attention_bwd: shape mismatch (head_dim must be 64 or 128)");
   TORCH_CHECK(lse.is_cuda() && lse.is_contiguous() && lse.scalar_type() == at::kFloat && lse.numel() == q.size(0) * q.size(1) * q.size(2), "attention_bwd: lse");
+  for (const at::Tensor* t : std::initializer_list<const at::Tensor*>{&k, &v, &out, &dout, &dq, &dk, &dv})
+    TORCH_CHECK(t->scalar_type() == q.scalar_type(), "attention_bwd: q, k, v, out, dout and the gradients must have one dtype");
   const c10::cuda::CUDAGuard guard(q.device());
   const int64_t B = q.size(0), Sq = q.size(1), Sk = k.size(1), H = q.size(2), D = q.size(3);
   const int64_t sq_pad = (Sq + 63) / 64 * 64;
@@ -725,7 +732,7 @@ void attention_bwd(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v
   PFX_CUDA_CHECK(pfx::attention_bwd(attn_view(q, "q"), attn_view(k, "k"), attn_view(v, "v"), attn_view(out, "out"), attn_view(dout, "dout"),
                                     lse.data_ptr<float>(), attn_view(dq, "dq"), attn_view(dk, "dk"), attn_view(dv, "dv"), dq_acc.data_ptr<float>(),
                                     stats[0].data_ptr<float>(), stats[1].data_ptr<float>(), (int)B, (int)Sq, (int)Sk, (int)H, (int)D, (float)scale,
-                                    causal, pfx::AttnDropout{(float)dropout_p, (uint64_t)seed}, cur_stream()));
+                                    causal, pfx::AttnDropout{(float)dropout_p, (uint64_t)seed}, dtype_code(q), cur_stream()));
 }
 
 at::Tensor attention_decode_packed(const at::Tensor& qkv, at::Tensor& k, at::Tensor& v, c10::optional<at::Tensor> mask, const at::Tensor& write_idx,
@@ -850,7 +857,7 @@ std::vector<at::Tensor> moe_tile_table(const at::Tensor& seg, int64_t e_local, i
 at::Tensor gemm_grouped(const at::Tensor& a, const at::Tensor& b, c10::optional<at::Tensor> bias, const at::Tensor& tile_group, at::Tensor& out,
                         bool b_kmajor, int64_t epilogue, c10::optional<at::Tensor> out2, c10::optional<at::Tensor> aux, int64_t row_align) {
   TORCH_CHECK(a.is_cuda() && a.dim() == 2 && b.dim() == 3 && a.is_contiguous() && b.is_contiguous() && out.is_contiguous(), "gemm_grouped: a [M,K], b [G,*,*] contiguous");
-  TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16 && out.scalar_type() == at::kBFloat16, "gemm_grouped: bf16 only");
+  TORCH_CHECK(is_16bit(a) && b.scalar_type() == a.scalar_type() && out.scalar_type() == a.scalar_type(), "gemm_grouped: bf16 or fp16 operands of one dtype");
   const int64_t M = a.size(0), K = a.size(1), G = b.size(0);
   const int64_t N = b_kmajor ? b.size(1) : b.size(2);
   TORCH_CHECK((b_kmajor ? b.size(2) : b.size(1)) == K, "gemm_grouped: K mismatch");
@@ -860,32 +867,32 @@ at::Tensor gemm_grouped(const at::Tensor& a, const at::Tensor& b, c10::optional<
   pfx::GemmArgs g{};
   g.a = a.data_ptr(); g.b = b.data_ptr(); g.d = out.data_ptr();
   if (bias.has_value() && bias->defined()) {
-    TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->numel() == G * N && bias->is_contiguous(), "gemm_grouped: bias [G, N] bf16");
+    TORCH_CHECK(bias->scalar_type() == a.scalar_type() && bias->numel() == G * N && bias->is_contiguous(), "gemm_grouped: bias [G, N] of the operands' dtype");
     g.bias = bias->data_ptr();
   } else {
     TORCH_CHECK(epilogue == pfx::EPI_NONE || epilogue == pfx::EPI_DGELU, "gemm_grouped: bias epilogue without bias");
   }
   if (epilogue == pfx::EPI_BIAS_GELU_DUAL) {
-    TORCH_CHECK(out2.has_value() && out2->is_contiguous() && out2->sizes() == out.sizes() && out2->scalar_type() == at::kBFloat16, "gemm_grouped: out2 like out");
+    TORCH_CHECK(out2.has_value() && out2->is_contiguous() && out2->sizes() == out.sizes() && out2->scalar_type() == a.scalar_type(), "gemm_grouped: out2 like out");
     g.d2 = out2->data_ptr();
   }
   if (epilogue == pfx::EPI_DGELU) {
-    TORCH_CHECK(aux.has_value() && aux->is_contiguous() && aux->sizes() == out.sizes() && aux->scalar_type() == at::kBFloat16, "gemm_grouped: aux like out");
+    TORCH_CHECK(aux.has_value() && aux->is_contiguous() && aux->sizes() == out.sizes() && aux->scalar_type() == a.scalar_type(), "gemm_grouped: aux like out");
     g.aux = aux->data_ptr(); g.ld_aux = (int)N;
   }
   g.M = (int)M; g.N = (int)N; g.K = (int)K;
   g.lda = (int)K; g.ldb = (int)(b_kmajor ? K : N); g.ldd = (int)N;
-  g.a_kmajor = true; g.b_kmajor = b_kmajor; g.out_mode = 0; g.epilogue = (int)epilogue; g.ab_format = 1; g.num_sms = num_sms(); g.config = 0;
+  g.a_kmajor = true; g.b_kmajor = b_kmajor; g.out_mode = 0; g.epilogue = (int)epilogue; g.ab_format = dtype_code(a); g.num_sms = num_sms(); g.config = 0;
   g.group.mode = 1; g.group.tile_group = tile_group.data_ptr<int>(); g.group.groups = (int)G; g.group.b_group_stride = (int)(b_kmajor ? N : K);
   g.group.row_align = (int)row_align;
   PFX_CUDA_CHECK(pfx::gemm_wgmma(g, cur_stream()));
   return out;
 }
 
-// Grouped expert wgrad: out[g] = dy[rows of g]^T . x[rows of g]   (dy [R, Mg], x [R, N], out [G, Mg, N] bf16; seg2 = (start, padded count) per expert)
+// Grouped expert wgrad: out[g] = dy[rows of g]^T . x[rows of g]   (dy [R, Mg], x [R, N], out [G, Mg, N], all bf16 or all fp16; seg2 = (start, padded count) per expert)
 at::Tensor gemm_grouped_wgrad(const at::Tensor& dy, const at::Tensor& x, const at::Tensor& seg2, at::Tensor& out) {
   TORCH_CHECK(dy.is_cuda() && dy.dim() == 2 && x.dim() == 2 && out.dim() == 3 && dy.is_contiguous() && x.is_contiguous() && out.is_contiguous(), "gemm_grouped_wgrad: contiguous");
-  TORCH_CHECK(dy.scalar_type() == at::kBFloat16 && x.scalar_type() == at::kBFloat16 && out.scalar_type() == at::kBFloat16, "gemm_grouped_wgrad: bf16 only");
+  TORCH_CHECK(is_16bit(dy) && x.scalar_type() == dy.scalar_type() && out.scalar_type() == dy.scalar_type(), "gemm_grouped_wgrad: bf16 or fp16 operands of one dtype");
   const int64_t R = dy.size(0), Mg = dy.size(1), N = x.size(1), G = out.size(0);
   TORCH_CHECK(x.size(0) == R && out.size(1) == Mg && out.size(2) == N && seg2.numel() == 2 * G && seg2.scalar_type() == at::kInt, "gemm_grouped_wgrad: shapes");
   TORCH_CHECK(Mg % 128 == 0 && N % 8 == 0, "gemm_grouped_wgrad: Mg % 128 == 0, N % 8 == 0");
@@ -894,7 +901,7 @@ at::Tensor gemm_grouped_wgrad(const at::Tensor& dy, const at::Tensor& x, const a
   g.a = dy.data_ptr(); g.b = x.data_ptr(); g.d = out.data_ptr();
   g.M = (int)(G * Mg); g.N = (int)N; g.K = (int)R;
   g.lda = (int)Mg; g.ldb = (int)N; g.ldd = (int)N;
-  g.a_kmajor = false; g.b_kmajor = false; g.out_mode = 0; g.epilogue = pfx::EPI_NONE; g.ab_format = 1; g.num_sms = num_sms(); g.config = 0;
+  g.a_kmajor = false; g.b_kmajor = false; g.out_mode = 0; g.epilogue = pfx::EPI_NONE; g.ab_format = dtype_code(dy); g.num_sms = num_sms(); g.config = 0;
   g.group.mode = 2; g.group.seg = seg2.data_ptr<int>(); g.group.groups = (int)G; g.group.m_per_group = (int)Mg;
   PFX_CUDA_CHECK(pfx::gemm_wgmma(g, cur_stream()));
   return out;

@@ -8,8 +8,8 @@
 // 16/32/64/128) and the accumulator fragment holds y^T — and K is split across the CTAs of a cluster so that
 // N/128 x kSplit CTAs pull weights through TMA concurrently.  The partial accumulators are reduced through
 // distributed shared memory: every CTA scatters 128/kSplit-row slices of its fp32 partial tile into the owning
-// CTA's smem (st.shared::cluster), one cluster barrier, and each owner sums its kSplit slices, adds the bias and
-// writes bf16 — no global workspace, no atomics, no second kernel.
+// CTA's smem (st.shared::cluster), one cluster barrier, and each owner sums its kSplit slices in fp32, adds the bias and
+// writes the operands' 16-bit type (bf16 or fp16, a template parameter) — no global workspace, no atomics, no second kernel.
 //
 // warp 4: TMA producer + barrier init, warps 0-3: one consumer warpgroup (products, then the reduction epilogue).
 // Reference call sites: the decode / prefill linears of GPTForGeneration (hybrid_model.py:1202-1339) run cuBLAS.
@@ -17,6 +17,7 @@
 #include "pfx_gemm.h"
 #include "pfx_kernels.h"
 #include <cudaTypedefs.h>
+#include <type_traits>
 
 namespace pfx {
 
@@ -39,6 +40,12 @@ struct SmallMSmem {
   static constexpr int kTotal = 1024 + kStages * kStageBytes + kRedBytes + kBarrierBytes;
 };
 
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+template <typename T> __device__ __forceinline__ T from_f32(float v);
+template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16(v); }
+template <> __device__ __forceinline__ __half from_f32<__half>(float v) { return __float2half_rn(v); }
+
 __device__ __forceinline__ void st_shared_cluster_f32(uint32_t addr, float v) {
   asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
 }
@@ -47,6 +54,7 @@ template <typename T, int kMPad, int kSplit>
 __global__ void __launch_bounds__(kSmThreads, 1)
 gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x, const T* __restrict__ bias,
                    T* __restrict__ y, int M, int N, int K, int ab_format) {
+  constexpr bool kBf16 = std::is_same<T, __nv_bfloat16>::value;   // fp16 otherwise; ab_format mirrors it for the host
   using S = SmallMSmem<kMPad>;
   constexpr int kStages = S::kStages;
   constexpr int kRowsPerOwner = kSmTileN / kSplit;
@@ -109,8 +117,8 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
 #pragma unroll
       for (int k = 0; k < kSmBlockK / kSmMmaK; ++k) {
         const uint64_t db = wgmma_desc(sb + k * kSmMmaK * 2, kDesc);
-        WgmmaSS<kMPad, true, 0, 0>::mma(acc[0], wgmma_desc(sa + k * kSmMmaK * 2, kDesc), db, 1u);      // bf16 only (checked by the host wrapper)
-        WgmmaSS<kMPad, true, 0, 0>::mma(acc[1], wgmma_desc(sa + 8192 + k * kSmMmaK * 2, kDesc), db, 1u);
+        WgmmaSS<kMPad, kBf16, 0, 0>::mma(acc[0], wgmma_desc(sa + k * kSmMmaK * 2, kDesc), db, 1u);
+        WgmmaSS<kMPad, kBf16, 0, 0>::mma(acc[1], wgmma_desc(sa + 8192 + k * kSmMmaK * 2, kDesc), db, 1u);
       }
       wgmma_commit();
       wgmma_wait<0>();
@@ -154,22 +162,23 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
       const int m = idx / kRowsPerOwner, nl = idx % kRowsPerOwner;
       const int n = row0 + nl;
       if (n >= N) continue;
-      float v = bias ? __bfloat162float(bias[n]) : 0.f;
+      float v = bias ? to_f32(bias[n]) : 0.f;
 #pragma unroll
       for (int s = 0; s < kSplit; ++s) v += red[(s * kMPad + m) * kRowsPerOwner + nl];
-      y[(size_t)m * N + n] = __float2bfloat16(v);
+      y[(size_t)m * N + n] = from_f32<T>(v);
     }
   }
 }
 
-template <int kMPad, int kSplit>
+template <typename T, int kMPad, int kSplit>
 cudaError_t launch_smallm(const void* x, const void* w, const void* bias, void* y, int M, int N, int K, cudaStream_t st) {
+  constexpr int dt = std::is_same<T, __nv_bfloat16>::value ? 1 : 0;
   using S = SmallMSmem<kMPad>;
   CUtensorMap tw, tx;
-  bool ok = make_tmap_2d(&tw, w, 2, 1, (uint64_t)K, (uint64_t)N, (uint64_t)K * 2, kSmBlockK, kSmTileN);
-  ok &= make_tmap_2d(&tx, x, 2, 1, (uint64_t)K, (uint64_t)M, (uint64_t)K * 2, kSmBlockK, kMPad);
+  bool ok = make_tmap_2d(&tw, w, 2, dt, (uint64_t)K, (uint64_t)N, (uint64_t)K * 2, kSmBlockK, kSmTileN);
+  ok &= make_tmap_2d(&tx, x, 2, dt, (uint64_t)K, (uint64_t)M, (uint64_t)K * 2, kSmBlockK, kMPad);
   if (!ok) return cudaErrorInvalidValue;
-  auto kern = gemm_smallm_kernel<__nv_bfloat16, kMPad, kSplit>;
+  auto kern = gemm_smallm_kernel<T, kMPad, kSplit>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal);
@@ -187,24 +196,32 @@ cudaError_t launch_smallm(const void* x, const void* w, const void* bias, void* 
   attr[0].val.clusterDim.x = kSplit; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kern, tw, tx, (const __nv_bfloat16*)bias, (__nv_bfloat16*)y, M, N, K, 1);
+  return cudaLaunchKernelEx(&cfg, kern, tw, tx, (const T*)bias, (T*)y, M, N, K, dt);
 }
 
-template <int kMPad>
+template <typename T, int kMPad>
 cudaError_t launch_split(const void* x, const void* w, const void* bias, void* y, int M, int N, int K, int split, cudaStream_t st) {
   switch (split) {
-    case 1: return launch_smallm<kMPad, 1>(x, w, bias, y, M, N, K, st);
-    case 2: return launch_smallm<kMPad, 2>(x, w, bias, y, M, N, K, st);
-    case 4: return launch_smallm<kMPad, 4>(x, w, bias, y, M, N, K, st);
-    default: return launch_smallm<kMPad, 8>(x, w, bias, y, M, N, K, st);
+    case 1: return launch_smallm<T, kMPad, 1>(x, w, bias, y, M, N, K, st);
+    case 2: return launch_smallm<T, kMPad, 2>(x, w, bias, y, M, N, K, st);
+    case 4: return launch_smallm<T, kMPad, 4>(x, w, bias, y, M, N, K, st);
+    default: return launch_smallm<T, kMPad, 8>(x, w, bias, y, M, N, K, st);
   }
+}
+
+template <typename T>
+cudaError_t launch_m(const void* x, const void* w, const void* bias, void* y, int M, int N, int K, int split, cudaStream_t st) {
+  if (M <= 16) return launch_split<T, 16>(x, w, bias, y, M, N, K, split, st);
+  if (M <= 32) return launch_split<T, 32>(x, w, bias, y, M, N, K, split, st);
+  if (M <= 64) return launch_split<T, 64>(x, w, bias, y, M, N, K, split, st);
+  return launch_split<T, 128>(x, w, bias, y, M, N, K, split, st);
 }
 
 }  // namespace
 
 cudaError_t gemm_smallm(const void* x, const void* w, const void* bias, void* y, int M, int N, int K, int dtype, int split, int num_sms,
                         cudaStream_t st) {
-  if (dtype != 1 || M < 1 || M > 128 || K % 8 || N % 8) return cudaErrorInvalidValue;
+  if ((dtype != 0 && dtype != 1) || M < 1 || M > 128 || K % 8 || N % 8) return cudaErrorInvalidValue;
   if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w)) & 15) return cudaErrorMisalignedAddress;
   if (split <= 0) {        // enough CTAs to cover the machine, but keep >= 4 k-blocks per CTA
     const int tiles = (N + kSmTileN - 1) / kSmTileN;
@@ -212,10 +229,7 @@ cudaError_t gemm_smallm(const void* x, const void* w, const void* bias, void* y,
     split = 1;
     while (split < 8 && tiles * split < num_sms && total_kb / (split * 2) >= 4) split *= 2;
   }
-  if (M <= 16) return launch_split<16>(x, w, bias, y, M, N, K, split, st);
-  if (M <= 32) return launch_split<32>(x, w, bias, y, M, N, K, split, st);
-  if (M <= 64) return launch_split<64>(x, w, bias, y, M, N, K, split, st);
-  return launch_split<128>(x, w, bias, y, M, N, K, split, st);
+  return dtype == 1 ? launch_m<__nv_bfloat16>(x, w, bias, y, M, N, K, split, st) : launch_m<__half>(x, w, bias, y, M, N, K, split, st);
 }
 
 }  // namespace pfx

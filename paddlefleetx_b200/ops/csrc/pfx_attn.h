@@ -5,7 +5,7 @@
 
 namespace pfx {
 
-// A [B, S, H, D] bf16 view with D contiguous; strides in elements.  Covers contiguous tensors, the q / k / v slices of a packed
+// A [B, S, H, D] 16-bit view with D contiguous; strides in elements.  Covers contiguous tensors, the q / k / v slices of a packed
 // [B, S, H, 3, D] projection output and sequence-major ([S, B, ...]) storage without any copy.
 struct AttnView {
   const void* ptr;
@@ -17,15 +17,16 @@ struct AttnDropout {
   uint64_t seed;      // counter-hash key; the element (b, h, q, k) keeps iff hash16(seed, b*H+h, q, k) >= p * 65536
 };
 
-// O = softmax(scale * Q K^T + causal) (dropout) V;  lse = row-wise log-sum-exp (natural log) [B, H, Sq] fp32
+// O = softmax(scale * Q K^T + causal) (dropout) V;  lse = row-wise log-sum-exp (natural log) [B, H, Sq] fp32.
+// dtype: 1 = bf16, 0 = fp16, for every view of the call (the flash kernels are compiled for both).
 cudaError_t attention_fwd_v2(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H,
-                             int D, float scale, bool causal, AttnDropout drop, cudaStream_t st);
+                             int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st);
 
 // Backward.  Workspace: dq_acc fp32 [B, Sq, H, D] (zeroed by the call), lse2 / delta fp32 [B, H, round_up(Sq, 64)].
-// dq / dk / dv may be strided views (e.g. slices of one packed [B, S, H, 3, D] gradient buffer).  D must be 128.
+// dq / dk / dv may be strided views (e.g. slices of one packed [B, S, H, 3, D] gradient buffer).  D is 64 or 128; dtype as above.
 cudaError_t attention_bwd(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, const AttnView& dout, const float* lse,
                           const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int Sq,
-                          int Sk, int H, int D, float scale, bool causal, AttnDropout drop, cudaStream_t st);
+                          int Sk, int H, int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st);
 
 // Evoformer gated attention (head width 32, H even): softmax(scale QK^T + mask_bias[g, k] + pair_bias[g / groups_per_pair, h, q, k]) V * sigmoid(gate).
 // q / out / gate [G, Sq, H, 32], k / v [G, Sk, H, 32] bf16 contiguous; mask_bias fp32 [G, Sk]; pair_bias bf16; lse fp32 [G, H, Sq].

@@ -150,6 +150,21 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
 }
+__device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {   // round to nearest; beyond 65504 the result is +-inf
+  __half2 v = __floats2half2_rn(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&v);
+}
+// 16-bit element type chosen at compile time: kBf16 = bf16, otherwise fp16
+template <bool kBf16>
+__device__ __forceinline__ uint32_t pack_16x2(float lo, float hi) {
+  if constexpr (kBf16) return pack_bf16x2(lo, hi);
+  else return pack_f16x2(lo, hi);
+}
+template <bool kBf16>
+__device__ __forceinline__ float2 load_16x2(const void* p) {   // two adjacent 16-bit values (4-byte aligned) as floats
+  if constexpr (kBf16) return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p));
+  else return __half22float2(*reinterpret_cast<const __half2*>(p));
+}
 __device__ __forceinline__ float gelu_tanh(float x) {
   // 0.5 x (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3)))
   const float k0 = 0.7978845608028654f, k1 = 0.044715f;

@@ -47,8 +47,15 @@ def _native_ok(*ts) -> bool:
     return t0.is_cuda and t0.dtype in _LOWP and _native.use_native(*ts)
 
 
+def tensor_core_dtype(*ts: Optional[torch.Tensor]) -> bool:
+    """True when every given tensor (``None`` entries are skipped) has one 16-bit dtype that the wgmma GEMM and flash-attention kernels
+    are compiled for: bf16 or fp16.  Mixed dtypes (fp16 activations with bf16 weights, say) are not; their callers fall back."""
+    dts = {t.dtype for t in ts if t is not None}
+    return len(dts) == 1 and next(iter(dts)) in _LOWP
+
+
 def _gemm_ok(x: torch.Tensor, *dims: int) -> bool:
-    return x.is_cuda and x.dtype == torch.bfloat16 and all(d % 8 == 0 for d in dims) and _native.use_native(x)
+    return x.is_cuda and tensor_core_dtype(x) and all(d % 8 == 0 for d in dims) and _native.use_native(x)
 
 
 # =============================================================================== linear
@@ -130,9 +137,8 @@ _FUSED_FFN = os.environ.get("PFX_FUSED_FFN", "1") == "1"
 def fused_ffn(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2: torch.Tensor, b2: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``gelu(x @ w1.T + b1) @ w2.T (+ b2)`` (tanh GELU).  The decoder layer passes ``b2 = None`` and folds that bias into its
     bias+dropout+residual kernel; expert FFNs pass it."""
-    if (_FUSED_FFN and x.is_cuda and x.dtype == torch.bfloat16 and w1.dtype == torch.bfloat16 and w2.dtype == torch.bfloat16 and b1 is not None
-            and b1.dtype == torch.bfloat16 and w1.is_contiguous() and w2.is_contiguous() and w1.shape[0] % 8 == 0 and w1.shape[1] % 8 == 0
-            and w2.shape[0] % 8 == 0 and x.numel() // x.shape[-1] > 128 and (b2 is None or b2.dtype == torch.bfloat16) and _native.use_native(x)):
+    if (_FUSED_FFN and x.is_cuda and b1 is not None and tensor_core_dtype(x, w1, b1, w2, b2) and w1.is_contiguous() and w2.is_contiguous() and w1.shape[0] % 8 == 0 and w1.shape[1] % 8 == 0
+            and w2.shape[0] % 8 == 0 and x.numel() // x.shape[-1] > 128 and _native.use_native(x)):
         return _FusedFFNFn.apply(x, w1, b1, w2, b2)
     return linear(bias_gelu(linear(x, w1, None), b1), w2, b2)
 
@@ -183,14 +189,14 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
         _count()
         y = _native.require().gemv_skinny(x.reshape(-1, x.shape[-1]).contiguous(), weight, bias)
         return y.view(*x.shape[:-1], weight.shape[0])
-    if (_SMALLM and x.is_cuda and x.dtype == torch.bfloat16 and weight.dtype == torch.bfloat16 and weight.is_contiguous()
+    if (_SMALLM and x.is_cuda and tensor_core_dtype(x, weight, bias) and weight.is_contiguous()
             and x.numel() // x.shape[-1] <= 128 and x.shape[-1] % 8 == 0 and weight.shape[0] % 8 == 0
             and not (torch.is_grad_enabled() and (x.requires_grad or weight.requires_grad)) and _native.available()):
         # prefill / batched decode: swap-AB wgmma GEMM, split-K over a cluster (csrc/gemm_smallm_sm90.cu)
         _count()
         y = _native.require().gemm_smallm(x.reshape(-1, x.shape[-1]).contiguous(), weight, bias, 0)
         return y.view(*x.shape[:-1], weight.shape[0])
-    if _gemm_ok(x, weight.shape[0], weight.shape[1]) and weight.dtype == torch.bfloat16 and weight.is_contiguous():
+    if _gemm_ok(x, weight.shape[0], weight.shape[1]) and tensor_core_dtype(x, weight) and weight.is_contiguous():
         return _LinearFn.apply(x, weight, bias)
     return F.linear(x, weight, bias)
 
@@ -311,7 +317,7 @@ def attention_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
 
 def matmul_nt(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     """a[M,K] @ b[N,K]^T without autograd (used by fused comm paths and inference)."""
-    if _gemm_ok(a, a.shape[-1], b.shape[0]):
+    if _gemm_ok(a, a.shape[-1], b.shape[0]) and tensor_core_dtype(a, b):
         _count()
         return _native.require().gemm(a, b, None, None, True, True, EPI_NONE, 0, 0)
     return a @ b.t()

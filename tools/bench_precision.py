@@ -1,0 +1,177 @@
+"""float16 against bfloat16 on the headline GPT-1.3B single-GPU step, and the kernels behind it, on one H100.
+
+    python tools/bench_precision.py --steps 20 --warmup 5            # arms fp16, bf16, fp16, bf16: one subprocess each
+    python tools/bench_precision.py --kernels                         # GEMM and flash-attention timings in both dtypes
+
+Step mode builds the exact configuration of ``bench.py --gpus 1`` (``bench.build_config``) and changes only
+``Engine.mix_precision.dtype``.  Each arm runs in its own process under bench.py's rules: W untimed warm-up steps, then K steps
+bracketed by synchronisation and CUDA events.  float16 trains with the dynamic loss scaler (initial scale ``scale_loss`` = 32768): the
+line reports the final scale and how many timed steps it skipped.  Every line carries the GPU name and power limit read in the same
+process (``nvidia-smi --query-gpu=name,power.limit``, read only).
+
+Kernel mode times the persistent GEMM at GPT-1.3B's Linear shapes (8 x 1024 tokens, hidden 2048: QKV, attention output, FFN1, FFN2 in the
+forward, dgrad and wgrad forms) and flash attention forward + backward at b 8, s 1024, h 16, d 128 (causal), in both dtypes.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+import types
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def gpu_info() -> dict:
+    try:
+        out = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
+                             timeout=10).stdout.strip()
+        name, power = [s.strip() for s in out.split(",")[:2]]
+        return dict(gpu=name, power_limit=power)
+    except Exception as e:          # the measurement still stands; say why the card is not named
+        return dict(gpu=None, power_limit=None, gpu_info_error=repr(e))
+
+
+def run_arm(dtype: str, steps: int, warmup: int) -> dict:
+    """One arm in this process: the headline GPT-1.3B single-GPU configuration of bench.py with ``Engine.mix_precision.dtype = dtype``,
+    ``warmup`` untimed steps, then ``steps`` steps between CUDA events.  Returns the JSON-ready result (ms/step, tokens/s, final loss, for
+    float16 the loss scale after the timed steps and how many of them the dynamic scaler skipped, and the GPU name and power limit)."""
+    import torch
+
+    import bench
+    from paddlefleetx_b200.core import EagerEngine
+    from paddlefleetx_b200.distributed.apis import env
+    from paddlefleetx_b200.models import build_module
+
+    assert torch.cuda.is_available(), "bench_precision.py needs a CUDA device"
+    args = types.SimpleNamespace(model="gpt-1.3b", layout="auto", local_batch=8, micro_batch=0, recompute="auto", seq_len=1024, layers=0,
+                                 step_overlap=-1, fused_tp=0, p2p=-1)
+    env.init_process_group("gpu")
+    torch.cuda.set_device(0)
+    cfg, lay = bench.build_config(args, 1)
+    cfg.Engine.mix_precision.dtype = dtype
+    env.init_dist_env(cfg)
+    env.set_seed(cfg.Global.seed)
+    engine = EagerEngine(configs=cfg, module=build_module(cfg))
+    dev = torch.device("cuda", 0)
+    assert next(engine._module.model.parameters()).dtype == getattr(torch, dtype)
+    seq, local, vocab = args.seq_len, lay["local"], cfg.Model.vocab_size
+    gen = torch.Generator().manual_seed(1234)
+    pool = []
+    for _ in range(4):
+        toks = torch.randint(0, vocab, (local, seq + 1), generator=gen, dtype=torch.int64)
+        pos = torch.arange(seq, dtype=torch.int64).unsqueeze(0).expand(local, seq).contiguous()
+        pool.append([t.to(dev) for t in (toks[:, :-1].contiguous(), pos, toks[:, 1:].contiguous(), torch.ones(local, seq))])
+    scaler = engine._scaler if dtype == "float16" else None
+
+    def device_step(i):
+        loss = engine._fit_impl(list(pool[i % len(pool)]))
+        engine._lr_scheduler.step(epoch=cfg.Global.global_batch_size)
+        engine._optimizer.clear_grad()
+        return loss
+
+    for i in range(warmup):
+        device_step(i)
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    skipped = 0
+    e0.record()
+    for i in range(steps):
+        loss = device_step(i)
+        if scaler is not None and scaler.found_inf:           # the scaler has already read the flag to the host inside step()
+            skipped += 1
+    e1.record()
+    torch.cuda.synchronize()
+    ms = e0.elapsed_time(e1) / steps
+    return dict(dtype=dtype, model="gpt-1.3b", steps=steps, warmup=warmup, ms_per_step=round(ms, 2),
+                tokens_per_s=round(local * seq / ms * 1e3, 1), final_loss=round(float(loss), 4),
+                loss_scale=scaler.get_scale() if scaler is not None else None, skipped_steps=skipped if scaler is not None else None, **gpu_info())
+
+
+def _time_ms(fn, iters=30, warmup=5) -> float:
+    import torch
+
+    for _ in range(warmup):
+        fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(iters):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / iters
+
+
+def run_kernels() -> list:
+    import torch
+
+    from paddlefleetx_b200.ops import _native
+
+    lib = _native.require()
+    tokens, h = 8 * 1024, 2048
+    linears = {"qkv": (3 * h, h), "attn_out": (h, h), "ffn1": (4 * h, h), "ffn2": (h, 4 * h)}     # (out, in) features
+    rows = []
+    info = gpu_info()
+    for dt in (torch.float16, torch.bfloat16):
+        torch.manual_seed(0)
+        for name, (n_out, n_in) in linears.items():
+            x = torch.randn(tokens, n_in, device="cuda", dtype=dt)
+            w = torch.randn(n_out, n_in, device="cuda", dtype=dt) * 0.02
+            dy = torch.randn(tokens, n_out, device="cuda", dtype=dt)
+            main_grad = torch.zeros(n_out, n_in, device="cuda")
+            forms = {"fwd": lambda: lib.gemm(x, w, None, None, True, True, 0, 0, 0),                  # y = x W^T
+                     "dgrad": lambda: lib.gemm(dy, w, None, None, True, False, 0, 0, 0),              # dx = dy W
+                     "wgrad": lambda: lib.gemm(dy, x, None, main_grad, False, False, 0, 2, 0)}        # main_grad += dy^T x
+            for form, fn in forms.items():
+                ms = _time_ms(fn)
+                rows.append(dict(kernel=f"gemm_{name}_{form}", dtype=str(dt).split(".")[-1], ms=round(ms, 4),
+                                 tflops=round(2.0 * tokens * n_out * n_in / ms / 1e9, 1), **info))
+        b, s, nh, d = 8, 1024, 16, 128
+        mix = torch.randn(b, s, nh, 3, d, device="cuda", dtype=dt)
+        q, k, v = mix.unbind(3)
+        dmix = torch.empty_like(mix)
+        dq, dk, dv = dmix.unbind(3)
+        go = torch.randn(b, s, nh, d, device="cuda", dtype=dt)
+        out, lse = lib.attention_fwd_v2(q, k, v, True, d ** -0.5, 0.0, 0)
+        flops = 4.0 * b * nh * s * s * d * 0.5
+        ms_f = _time_ms(lambda: lib.attention_fwd_v2(q, k, v, True, d ** -0.5, 0.0, 0))
+        ms_b = _time_ms(lambda: lib.attention_bwd(q, k, v, out, go, lse, dq, dk, dv, True, d ** -0.5, 0.0, 0))
+        rows.append(dict(kernel="attention_fwd_b8_s1024_h16_d128_causal", dtype=str(dt).split(".")[-1], ms=round(ms_f, 4),
+                         tflops=round(flops / ms_f / 1e9, 1), **info))
+        rows.append(dict(kernel="attention_bwd_b8_s1024_h16_d128_causal", dtype=str(dt).split(".")[-1], ms=round(ms_b, 4),
+                         tflops=round(2.5 * flops / ms_b / 1e9, 1), **info))
+    return rows
+
+
+def main():
+    p = argparse.ArgumentParser()
+    p.add_argument("--steps", type=int, default=20)
+    p.add_argument("--warmup", type=int, default=5)
+    p.add_argument("--rounds", type=int, default=2, help="fp16 / bf16 pairs, alternated")
+    p.add_argument("--kernels", action="store_true", help="time the GEMM and attention kernels instead of the training step")
+    p.add_argument("--arm", default=None, choices=["float16", "bfloat16"], help=argparse.SUPPRESS)
+    a = p.parse_args()
+    if a.kernels:
+        for row in run_kernels():
+            print(json.dumps(row), flush=True)
+        return
+    if a.arm:
+        print(json.dumps(run_arm(a.arm, a.steps, a.warmup)), flush=True)
+        return
+    for _ in range(a.rounds):
+        for dtype in ("float16", "bfloat16"):
+            res = subprocess.run([sys.executable, os.path.abspath(__file__), "--arm", dtype, "--steps", str(a.steps), "--warmup", str(a.warmup)],
+                                 capture_output=True, text=True)
+            line = next((l for l in reversed(res.stdout.splitlines()) if l.startswith("{")), None)
+            if res.returncode != 0 or line is None:
+                sys.stderr.write(res.stdout[-4000:] + res.stderr[-4000:])
+                raise SystemExit(f"{dtype} arm failed with exit code {res.returncode}")
+            print(line, flush=True)
+
+
+if __name__ == "__main__":
+    main()

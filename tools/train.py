@@ -48,3 +48,4 @@ def main(argv=None):
 
 if __name__ == "__main__":
     main()
+    env.destroy_process_group()
