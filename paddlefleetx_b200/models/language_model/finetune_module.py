@@ -4,6 +4,7 @@ automatic fused<->split QKV conversion, loss and metric selected by name from th
 from __future__ import annotations
 
 import os
+from typing import Optional
 
 import torch
 import torch.nn.functional as F
@@ -17,27 +18,31 @@ _LOSSES = {"CrossEntropyLoss": lambda logits, y: F.cross_entropy(logits.float(),
            "MSELoss": lambda logits, y: F.mse_loss(logits.float().reshape(-1), y.float().reshape(-1))}
 
 
-def convert_qkv_layout(state: dict, fuse: bool, num_heads: int) -> dict:
+def convert_qkv_layout(state: dict, fuse: bool, num_heads: int, num_kv_heads: Optional[int] = None) -> dict:
     """Fuse ``q_proj/k_proj/v_proj`` into ``qkv_proj`` ([heads, 3, head_dim] rows) or split it back
-    (reference language_module.py:312-383, transposed to our [out, in] storage)."""
+    (reference language_module.py:312-383, transposed to our [out, in] storage).  With ``num_kv_heads`` K/V heads (grouped-query
+    attention, default ``num_heads``) the fused rows are ``[kv_heads, G + 2, head_dim]``: the G query heads of a group, its key, its value."""
+    kvh = num_kv_heads or num_heads
+    g = num_heads // kvh
     out = dict(state)
     if fuse:
         for k in [k for k in state if k.endswith("q_proj.weight") or k.endswith("q_proj.bias")]:
             base, kind = k.rsplit("q_proj.", 1)
             q, kk, v = state[base + "q_proj." + kind], state[base + "k_proj." + kind], state[base + "v_proj." + kind]
             hd = q.shape[0] // num_heads
-            parts = [t.reshape(num_heads, 1, hd, *t.shape[1:]) for t in (q, kk, v)]
-            out[base + "qkv_proj." + kind] = torch.cat(parts, 1).reshape(3 * q.shape[0], *q.shape[1:])
+            parts = [t.reshape(kvh, n, hd, *t.shape[1:]) for t, n in ((q, g), (kk, 1), (v, 1))]
+            out[base + "qkv_proj." + kind] = torch.cat(parts, 1).reshape(q.shape[0] + 2 * kk.shape[0], *q.shape[1:])
             for n in ("q_proj.", "k_proj.", "v_proj."):
                 out.pop(base + n + kind)
     else:
         for k in [k for k in state if "qkv_proj." in k]:
             base, kind = k.rsplit("qkv_proj.", 1)
             w = state[k]
-            hd = w.shape[0] // (3 * num_heads)
-            w = w.reshape(num_heads, 3, hd, *w.shape[1:])
-            for i, n in enumerate(("q_proj.", "k_proj.", "v_proj.")):
-                out[base + n + kind] = w[:, i].reshape(num_heads * hd, *w.shape[3:])
+            hd = w.shape[0] // (num_heads + 2 * kvh)
+            w = w.reshape(kvh, g + 2, hd, *w.shape[1:])
+            out[base + "q_proj." + kind] = w[:, :g].reshape(num_heads * hd, *w.shape[3:])
+            for i, n in ((g, "k_proj."), (g + 1, "v_proj.")):
+                out[base + n + kind] = w[:, i].reshape(kvh * hd, *w.shape[3:])
             out.pop(k)
     return out
 
@@ -76,7 +81,8 @@ class GPTFinetuneModule(LanguageModule):
             state = torch.load(path, map_location="cpu", weights_only=False)
             fused_ckpt = any("qkv_proj" in k for k in state)
             if fused_ckpt != bool(cfg.Model.get("fuse_attn_qkv", True)):
-                state = convert_qkv_layout(state, bool(cfg.Model.get("fuse_attn_qkv", True)), cfg.Model.num_attention_heads)
+                state = convert_qkv_layout(state, bool(cfg.Model.get("fuse_attn_qkv", True)), cfg.Model.num_attention_heads,
+                                           cfg.Model.get("num_key_value_heads"))
             own = model.state_dict()
             load = {k: v.to(own[k].dtype) for k, v in state.items() if k in own and own[k].shape == v.shape}
             missing = [k for k in own if k not in load]

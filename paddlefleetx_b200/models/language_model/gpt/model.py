@@ -13,7 +13,10 @@ Capabilities mirrored from the reference (single-card ``gpt/dygraph/single_model
 State-dict keys keep the reference's structured names (SURVEY §5.4), e.g.
 ``gpt.decoder.layers.3.self_attn.qkv_proj.weight``; linear weights are stored ``[out, in]`` (torch) instead
 of Paddle's ``[in, out]`` — ``utils/ckpt_convert.py`` transposes when importing genuine Paddle checkpoints.
-The fused-QKV output dimension is laid out ``[heads, 3, head_dim]`` like the reference.
+The fused-QKV output dimension is laid out ``[heads, 3, head_dim]`` like the reference.  With grouped-query attention
+(``num_key_value_heads`` = Hkv < heads, G = heads / Hkv query heads per K/V head) it is ``[Hkv, G + 2, head_dim]``: the G query heads of
+a group, then its key, then its value.  G = 1 is the ``[heads, 3, head_dim]`` layout, and because the layout splits by whole groups
+along the output rows, tensor parallelism shards it like any column-parallel weight when ``Hkv % mp == 0``.
 """
 from __future__ import annotations
 
@@ -82,7 +85,8 @@ def make_norm(kind: Optional[str], hidden: int, sequence_parallel: bool = False,
 
 class KVCache:
     """Pre-allocated static KV cache: in-place writes, no per-step concat/re-allocation (the reference grows
-    its cache with ``concat`` every token, hybrid_model.py:198-214)."""
+    its cache with ``concat`` every token, hybrid_model.py:198-214).  ``heads`` are the K/V heads (fewer than the query heads under
+    grouped-query attention)."""
 
     def __init__(self, batch: int, max_len: int, heads: int, head_dim: int, dtype, device):
         self.k = torch.zeros(batch, max_len, heads, head_dim, dtype=dtype, device=device)
@@ -112,14 +116,19 @@ class MultiHeadAttention(nn.Module):
     def __init__(self, hidden: int, num_heads: int, attn_dropout: float = 0.0, fuse_attn_qkv: bool = True, scale_qk_coeff: float = 1.0,
                  use_flash_attn: bool = True, fused_softmax_with_triangular: bool = True, sequence_parallel: bool = False,
                  mp_group=None, init_std: float = 0.02, out_init_std: float = 0.02, recompute_core: bool = False,
-                 fused_tp_comm: bool = False, use_rope: bool = False, dtype=None, device=None):
+                 fused_tp_comm: bool = False, use_rope: bool = False, num_key_value_heads: Optional[int] = None, dtype=None, device=None):
         super().__init__()
         self.hidden, self.num_heads = hidden, num_heads
         self.head_dim = hidden // num_heads
         assert self.head_dim * num_heads == hidden
+        self.num_kv_heads = num_key_value_heads or num_heads
+        assert num_heads % self.num_kv_heads == 0, f"heads {num_heads} % num_key_value_heads {self.num_kv_heads}"
+        self.group = num_heads // self.num_kv_heads            # query heads per K/V head
         self.world = C.group_size(mp_group)
         assert num_heads % self.world == 0, f"heads {num_heads} % mp {self.world}"
+        assert self.num_kv_heads % self.world == 0, f"num_key_value_heads {self.num_kv_heads} % mp {self.world}"
         self.local_heads = num_heads // self.world
+        self.local_kv_heads = self.num_kv_heads // self.world
         self.attn_dropout = attn_dropout
         self.fuse_attn_qkv = fuse_attn_qkv
         self.scale_qk_coeff = scale_qk_coeff
@@ -136,12 +145,13 @@ class MultiHeadAttention(nn.Module):
         if sequence_parallel:
             ckw["fused_comm"] = fused_tp_comm
             rkw["fused_comm"] = fused_tp_comm
+        kv_width = self.num_kv_heads * self.head_dim
         if fuse_attn_qkv:
-            self.qkv_proj = Col(hidden, 3 * hidden, **ckw)
+            self.qkv_proj = Col(hidden, hidden + 2 * kv_width, **ckw)
         else:
             self.q_proj = Col(hidden, hidden, **ckw)
-            self.k_proj = Col(hidden, hidden, **ckw)
-            self.v_proj = Col(hidden, hidden, **ckw)
+            self.k_proj = Col(hidden, kv_width, **ckw)
+            self.v_proj = Col(hidden, kv_width, **ckw)
         self.out_proj = Row(hidden, hidden, **rkw)
         # context parallelism (``Distributed.cp_degree`` > 1): the group comes from the process topology, not from a constructor argument,
         # because to every other part of the model the members of a cp group are ordinary data-parallel ranks
@@ -150,21 +160,33 @@ class MultiHeadAttention(nn.Module):
 
         hcg = getattr(_env, "_hcg", None)           # only an already-built topology counts (get_hcg() would build a default one)
         if hcg is not None and getattr(hcg, "cp", 1) > 1:
+            if self.group > 1:
+                raise ValueError("num_key_value_heads < num_attention_heads is not supported with context parallelism (Distributed.cp_degree > 1)")
             self.cp_group = hcg.get_context_parallel_group()
             self.cp_mode = getattr(hcg, "cp_mode", "ulysses")
             assert self.cp_mode == "ring" or self.local_heads % self.cp_group.nranks == 0, \
                 f"local heads {self.local_heads} % cp {self.cp_group.nranks} (Ulysses shards heads; cp_mode: ring has no such limit)"
 
     # -- projections -------------------------------------------------------------------------
+    def _packed_view(self, mix: torch.Tensor) -> torch.Tensor:
+        """fused projection output -> ``[.., local_kv_heads, G + 2, d]`` (``[.., local_heads, 3, d]`` without grouping)."""
+        return mix.view(*mix.shape[:-1], self.local_kv_heads, self.group + 2, self.head_dim)
+
+    def _split_packed(self, mix: torch.Tensor):
+        """q ``[.., local_heads, d]``, k / v ``[.., local_kv_heads, d]`` from the packed view."""
+        if self.group == 1:
+            return mix.unbind(-2)
+        g = self.group
+        return mix[..., :g, :].flatten(-3, -2), mix[..., g, :], mix[..., g + 1, :]
+
     def _qkv(self, x: torch.Tensor):
-        """returns q, k, v as ``[b, s, local_heads, d]``."""
+        """returns q as ``[b, s, local_heads, d]`` and k, v as ``[b, s, local_kv_heads, d]``."""
         if self.fuse_attn_qkv:
-            mix = self.qkv_proj(x)
-            mix = mix.view(*mix.shape[:-1], self.local_heads, 3, self.head_dim)
-            q, k, v = mix.unbind(-2)
+            q, k, v = self._split_packed(self._packed_view(self.qkv_proj(x)))
         else:
-            q, k, v = (p(x).view(*x.shape[:-1] if not self.sequence_parallel else (-1, x.shape[1]), self.local_heads, self.head_dim)
-                       for p in (self.q_proj, self.k_proj, self.v_proj))
+            lead = x.shape[:-1] if not self.sequence_parallel else (-1, x.shape[1])
+            q, k, v = (p(x).view(*lead, n, self.head_dim)
+                       for p, n in ((self.q_proj, self.local_heads), (self.k_proj, self.local_kv_heads), (self.v_proj, self.local_kv_heads)))
         if self.sequence_parallel:      # [s, b, heads, d] -> [b, s, heads, d]
             q, k, v = (t.transpose(0, 1) for t in (q, k, v))
         return q, k, v
@@ -237,8 +259,7 @@ class MultiHeadAttention(nn.Module):
                 and not (self.recompute_core and self.training)):
             # fused projection output [.., heads, 3, d] goes to the flash kernels as it is: q / k / v are read in place (TMA views), the
             # backward writes one packed gradient — no unbind / transpose / cat copies around the attention
-            mix = self.qkv_proj(x)
-            mix = mix.view(*mix.shape[:-1], self.local_heads, 3, self.head_dim)
+            mix = self._packed_view(self.qkv_proj(x))
             if self.sequence_parallel:
                 mix = mix.transpose(0, 1)
             if mix.shape[1] > 1:
@@ -252,7 +273,7 @@ class MultiHeadAttention(nn.Module):
             else:
                 out = None
             if out is None:
-                q, k, v = mix.unbind(-2)
+                q, k, v = self._split_packed(mix)
                 out = self._core(q, k, v, None)
             out = out.reshape(out.shape[0], out.shape[1], self.local_heads * self.head_dim)
             if self.sequence_parallel:
@@ -336,7 +357,7 @@ class TransformerDecoderLayer(nn.Module):
         b = x.shape[0]
         x2 = x.reshape(b, -1)
         qkv = OF.gemv_fused(x2, a.qkv_proj.weight, a.qkv_proj.bias, ln=(self.norm1.weight, self.norm1.bias, self.norm1.eps))
-        o = OF.attention_decode_packed(qkv.view(b, 1, a.local_heads, 3, a.head_dim), cache.k, cache.v, attn_mask, cache.static_index,
+        o = OF.attention_decode_packed(qkv.view(b, 1, a.local_kv_heads, a.group + 2, a.head_dim), cache.k, cache.v, attn_mask, cache.static_index,
                                        1.0 / math.sqrt(a.head_dim))
         x2 = OF.gemv_fused(o.view(b, -1), a.out_proj.weight, a.out_proj.bias, residual=x2)
         h = OF.gemv_fused(x2, self.linear1.weight, self.linear1.bias, ln=(self.norm2.weight, self.norm2.bias, self.norm2.eps), act="gelu")
@@ -419,7 +440,7 @@ class GPTModel(nn.Module):
                  fused_linear: bool = False, fuse_attn_qkv: bool = True, scale_qk_by_layer_num: bool = True,
                  sequence_parallel: bool = False, use_flash_attn: bool = True, fused_softmax_with_triangular: bool = True,
                  mp_group=None, moe_configs: Optional[dict] = None, fused_tp_comm: bool = False, use_rope: bool = False,
-                 normalization: Optional[str] = None, dtype=None, device=None, **unused):
+                 normalization: Optional[str] = None, num_key_value_heads: Optional[int] = None, dtype=None, device=None, **unused):
         super().__init__()
         ffn_hidden_size = ffn_hidden_size or 4 * hidden_size
         recompute_granularity = recompute_granularity or "full"
@@ -444,13 +465,14 @@ class GPTModel(nn.Module):
                 recompute_core=use_recompute and recompute_granularity == "core_attn", moe_layer=moe, fused_tp_comm=fused_tp_comm,
                 dtype=dtype, device=device, fuse_attn_qkv=fuse_attn_qkv,
                 scale_qk_coeff=float(num_layers) if scale_qk_by_layer_num else 1.0, use_flash_attn=use_flash_attn,
-                fused_softmax_with_triangular=fused_softmax_with_triangular, use_rope=use_rope, normalization=normalization))
+                fused_softmax_with_triangular=fused_softmax_with_triangular, use_rope=use_rope, normalization=normalization,
+                num_key_value_heads=num_key_value_heads))
         self.decoder = TransformerDecoder(layers, hidden_size, use_recompute, recompute_granularity, no_recompute_layers, sp, dtype, device,
                                           normalization=normalization)
 
     def new_caches(self, batch: int, max_len: int) -> List[KVCache]:
         p = self.decoder.norm.weight
-        lh, hd = self.decoder.layers[0].self_attn.local_heads, self.decoder.layers[0].self_attn.head_dim
+        lh, hd = self.decoder.layers[0].self_attn.local_kv_heads, self.decoder.layers[0].self_attn.head_dim
         return [KVCache(batch, max_len, lh, hd, p.dtype, p.device) for _ in self.decoder.layers]
 
     def forward(self, input_ids, position_ids=None, attention_mask=None, caches: Optional[List[KVCache]] = None):

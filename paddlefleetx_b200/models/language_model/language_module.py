@@ -9,6 +9,7 @@ log line is kept verbatim because the TIPC-style harness greps it.
 from __future__ import annotations
 
 import copy
+from typing import Optional
 
 import torch
 
@@ -102,8 +103,10 @@ def process_configs(config):
     return config
 
 
-def get_model_size(l: int, h: int, v: int, s: int) -> float:
-    p = (v + s) * h + (4 * h * h + 4 * h) * l + (2 * (2 * h)) * l + (8 * h * h + 5 * h) * l + 2 * h
+def get_model_size(l: int, h: int, v: int, s: int, kv_hidden: Optional[int] = None) -> float:
+    """Parameter count; ``kv_hidden`` = K/V heads x head_dim (grouped-query attention), default ``h``: QKV is h (h + 2 kv_hidden)."""
+    kv = h if kv_hidden is None else kv_hidden
+    p = (v + s) * h + (2 * h * h + 2 * h * kv + 2 * h + 2 * kv) * l + (2 * (2 * h)) * l + (8 * h * h + 5 * h) * l + 2 * h
     logger.info("Model Size: {:.2f} B".format(p / 1e9))
     return p
 
@@ -111,7 +114,8 @@ def get_model_size(l: int, h: int, v: int, s: int) -> float:
 _MODEL_KEYS = ("vocab_size", "hidden_size", "num_layers", "num_attention_heads", "ffn_hidden_size", "hidden_dropout_prob",
                "attention_probs_dropout_prob", "max_position_embeddings", "type_vocab_size", "initializer_range", "use_recompute",
                "recompute_granularity", "no_recompute_layers", "fused_linear", "fuse_attn_qkv", "scale_qk_by_layer_num",
-               "sequence_parallel", "use_flash_attn", "fused_softmax_with_triangular", "moe_configs", "use_rope", "normalization", "virtual_pp_degree")
+               "sequence_parallel", "use_flash_attn", "fused_softmax_with_triangular", "moe_configs", "use_rope", "normalization", "virtual_pp_degree",
+               "num_key_value_heads")
 
 
 def model_kwargs(config) -> dict:
@@ -245,7 +249,8 @@ class GPTModule(LanguageModule):
         cfg.Model["vocab_size"] = vocab
         kw = model_kwargs(cfg)
         kw["vocab_size"] = vocab
-        get_model_size(kw["num_layers"], kw["hidden_size"], vocab, kw.get("max_position_embeddings", 1024))
+        kv_hidden = kw["hidden_size"] // kw["num_attention_heads"] * kw["num_key_value_heads"] if kw.get("num_key_value_heads") else None
+        get_model_size(kw["num_layers"], kw["hidden_size"], vocab, kw.get("max_position_embeddings", 1024), kv_hidden)
         dtype, device = _param_dtype(cfg), _device(cfg)
         fused_tp = bool(cfg.get("Fused", {}).get("tp_comm", False))
         if d.pp_degree > 1:

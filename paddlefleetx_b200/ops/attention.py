@@ -1,11 +1,14 @@
 """Attention front-end.
 
 ``attention(q, k, v)`` takes ``[b, s, heads, d]`` tensors (views are fine: the slices of a packed QKV projection, sequence-major
-storage).  Path selection on CUDA / bf16 or fp16 (q, k and v of one dtype):
+storage).  k and v may have fewer heads than q (grouped-query attention: ``heads % kv_heads == 0``, query head ``h`` attends with K/V
+head ``h // (heads // kv_heads)``, the convention of ``repeat_interleave``).  Path selection on CUDA / bf16 or fp16 (q, k and v of one
+dtype):
   * training and inference at head_dim 128 or 64: our wgmma flash kernels — ``csrc/attention_fwd_sm90.cu`` and
     ``csrc/attention_bwd_sm90.cu`` — with in-kernel causal masking and counter-hash dropout (the backward regenerates the mask; nothing is
-    stored).  ``flash_attention_packed`` is the same pair for the ``[b, s, heads, 3, d]`` output of a fused QKV projection: it reads q / k / v
-    in place and writes ONE packed gradient, so no split / cat copies surround the kernels,
+    stored).  ``flash_attention_packed`` is the same pair for the ``[b, s, heads, 3, d]`` output of a fused QKV projection (``[b, s,
+    kv_heads, G + 2, d]`` with grouped K/V: the G query heads of a group, then its key and value): it reads q / k / v in place and writes
+    ONE packed gradient, so no split / cat copies surround the kernels,
   * single-query decode steps over the static KV cache use ``csrc/attention_decode.cu`` (see models/.../gpt/model.py),
   * explicit masks, other head sizes, mixed dtypes, fp32 and CPU tensors: PyTorch SDPA — a *library* call, reported as such by the launch
     accounting (it does not count towards ``gpu_launches``); ``PFX_NATIVE_ATTN=0`` forces it everywhere,
@@ -26,6 +29,11 @@ _NATIVE = int(os.environ.get("PFX_NATIVE_ATTN", "1"))
 _MASK64 = (1 << 64) - 1
 
 
+def _q_heads(q: torch.Tensor) -> int:
+    """Query heads of ``[b, s, heads, d]`` or of the ``[b, s, kv_heads, G, d]`` query part of a grouped packed projection."""
+    return q.shape[2] * q.shape[3] if q.dim() == 5 else q.shape[2]
+
+
 def _native_ok(q, k, v, attn_mask, causal, needs_grad: bool) -> bool:
     from .functional import tensor_core_dtype
 
@@ -34,8 +42,10 @@ def _native_ok(q, k, v, attn_mask, causal, needs_grad: bool) -> bool:
     d = q.shape[-1]
     if d not in (64, 128) or q.shape[1] < 1 or (causal and k.shape[1] < q.shape[1]):
         return False
+    if k.dim() != 4 or v.shape != k.shape or _q_heads(q) % k.shape[2] or (q.dim() == 5 and q.shape[2] != k.shape[2]):
+        return False
     for t in (q, k, v):
-        if t.dim() != 4 or t.stride(3) != 1 or any(t.stride(i) % 8 for i in range(3)) or t.data_ptr() % 16:
+        if t.dim() not in (4, 5) or t.stride(-1) != 1 or any(t.stride(i) % 8 for i in range(t.dim() - 1)) or t.data_ptr() % 16:
             return False
     from . import _native
 
@@ -75,9 +85,19 @@ def attn_keep_mask(seed: int, B: int, H: int, Sq: int, Sk: int, p: float, device
     return keep.view(B, H, Sq, Sk)
 
 
+def _split_packed(mix: torch.Tensor):
+    """q / k / v views of a ``[b, s, kv_heads, G + 2, d]`` projection output: q is ``[b, s, heads, d]`` for G = 1 (the ``[.., 3, d]``
+    layout) and ``[b, s, kv_heads, G, d]`` otherwise (no uniform head stride; the kernels take it as it is)."""
+    g = mix.shape[3] - 2
+    if g == 1:
+        return mix.unbind(3)
+    return mix[:, :, :, :g], mix[:, :, :, g], mix[:, :, :, g + 1]
+
+
 class _FlashAttnFn(torch.autograd.Function):
-    """q / k / v ``[b, s, h, d]`` views -> ``[b, s, h, d]``.  ``packed`` = the three are slices of one ``[b, s, h, 3, d]`` tensor, which is
-    then the single differentiable input (and the single gradient: dq / dk / dv are written straight into its three slices)."""
+    """q / k / v ``[b, s, h, d]`` views (k / v may have fewer heads) -> ``[b, s, h, d]``.  ``packed`` = the three are slices of one
+    ``[b, s, kv_heads, G + 2, d]`` tensor, which is then the single differentiable input (and the single gradient: dq / dk / dv are
+    written straight into its slices)."""
 
     @staticmethod
     def forward(ctx, packed, q, k, v, causal, scale, dropout_p, seed):
@@ -85,7 +105,7 @@ class _FlashAttnFn(torch.autograd.Function):
         from . import functional as OF
 
         if packed is not None:
-            q, k, v = packed.unbind(3)
+            q, k, v = _split_packed(packed)
         out, lse = _native.require().attention_fwd_v2(q, k, v, bool(causal), float(scale), float(dropout_p), int(seed))
         OF._count()
         ctx.save_for_backward(q, k, v, out, lse)
@@ -103,9 +123,9 @@ class _FlashAttnFn(torch.autograd.Function):
             dout = dout.contiguous()
         dmix = None
         if is_packed:
-            b, s, h, d = q.shape
-            dmix = torch.empty(b, s, h, 3, d, dtype=q.dtype, device=q.device)
-            dq, dk, dv = dmix.unbind(3)
+            b, s, hkv, d = k.shape
+            dmix = torch.empty(b, s, hkv, _q_heads(q) // hkv + 2, d, dtype=q.dtype, device=q.device)
+            dq, dk, dv = _split_packed(dmix)
         else:
             dq, dk, dv = torch.empty_like(q, memory_format=torch.contiguous_format), torch.empty_like(k, memory_format=torch.contiguous_format), \
                 torch.empty_like(v, memory_format=torch.contiguous_format)
@@ -117,16 +137,17 @@ class _FlashAttnFn(torch.autograd.Function):
 
 
 def flash_attention_packed(mix: torch.Tensor, causal: bool = True, dropout_p: float = 0.0, scale: Optional[float] = None) -> Optional[torch.Tensor]:
-    """Attention on the ``[b, s, heads, 3, d]`` view of a fused QKV projection output (any batch / sequence strides).  Returns ``None`` when
-    the native kernels do not apply (caller falls back to ``attention`` on the unbound slices)."""
-    if mix.dim() != 5 or mix.shape[3] != 3:
+    """Attention on the ``[b, s, heads, 3, d]`` view of a fused QKV projection output (any batch / sequence strides), or on its grouped form
+    ``[b, s, kv_heads, G + 2, d]``.  Returns ``None`` when the native kernels do not apply (caller falls back to ``attention`` on the
+    slices)."""
+    if mix.dim() != 5 or mix.shape[3] < 3:
         return None
-    q, k, v = mix.unbind(3)
+    q, k, v = _split_packed(mix)
     needs_grad = torch.is_grad_enabled() and mix.requires_grad
     if not _native_ok(q, k, v, None, causal, needs_grad):
         return None
     sc = float(scale if scale is not None else q.shape[-1] ** -0.5)
-    seed = _dropout_seed(dropout_p, q.shape[0] * q.shape[2] * q.shape[1] * k.shape[1])
+    seed = _dropout_seed(dropout_p, q.shape[0] * _q_heads(q) * q.shape[1] * k.shape[1])
     return _FlashAttnFn.apply(mix, None, None, None, causal, sc, dropout_p, seed)
 
 
@@ -140,16 +161,20 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = 
     qt, kt, vt = (t.transpose(1, 2) for t in (q, k, v))           # [b, h, s, d]
     if attn_mask is not None:
         causal = False
-    out = F.scaled_dot_product_attention(qt, kt, vt, attn_mask=attn_mask, dropout_p=dropout_p, is_causal=causal, scale=scale)
+    gqa = {"enable_gqa": True} if k.shape[2] != q.shape[2] else {}
+    out = F.scaled_dot_product_attention(qt, kt, vt, attn_mask=attn_mask, dropout_p=dropout_p, is_causal=causal, scale=scale, **gqa)
     return out.transpose(1, 2)
 
 
 def core_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: float, dropout_p: float, training: bool,
                    attn_mask: Optional[torch.Tensor] = None, causal: bool = True, rng_name: Optional[str] = "local_seed"
                    ) -> torch.Tensor:
-    """Unfused attention: scores materialised as ``[b, heads, sq, sk]``."""
+    """Unfused attention: scores materialised as ``[b, heads, sq, sk]``.  Grouped K/V heads are repeated to the query heads."""
     from . import functional as OF
 
+    if k.shape[2] != q.shape[2]:
+        g = q.shape[2] // k.shape[2]
+        k, v = k.repeat_interleave(g, dim=2), v.repeat_interleave(g, dim=2)
     qt, kt, vt = (t.transpose(1, 2) for t in (q, k, v))
     scores = torch.matmul(qt, kt.transpose(-1, -2))
     if attn_mask is None and causal:

@@ -75,13 +75,18 @@ struct BwParams {
   uint32_t drop_thresh16;              // 0 = no dropout
   float inv_keep;
   uint64_t seed;
+  int G, gs_q;                         // grouped-query instantiation only: query heads per K/V head, q stride between groups
 };
 
 __device__ __forceinline__ void tma_tile(const CUtensorMap* m, bool swapped, uint32_t bar, uint32_t dst, int col, int s, int b) {
   if (swapped) tma_load_3d(m, bar, dst, col, b, s); else tma_load_3d(m, bar, dst, col, s, b);
 }
 
-template <int kHd, bool kBf16>   // kBf16: bf16 operands and gradients, otherwise fp16
+// kBf16: bf16 operands and gradients, otherwise fp16.  kGqa: G = H / Hkv > 1 query heads share one K/V head (a separate instantiation,
+// so the multi-head kernels are compiled exactly as without it).  The CTA then owns a key tile of one (batch, K/V head) and walks the
+// query tiles of all G heads of the group in turn, with each head's lse / delta, dropout key, Q column and dQ column, while dK / dV
+// stay in registers: they are exact sums written once, with no atomics, and deterministic.
+template <int kHd, bool kBf16, bool kGqa>
 __global__ void __launch_bounds__(kBwThreads, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v,
                      const __grid_constant__ CUtensorMap tmap_do, const __grid_constant__ CUtensorMap tmap_dq, const __grid_constant__ BwParams prm) {
@@ -103,14 +108,19 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
   // into the same dQ rows run at the same time and meet in L2.  Within a head the tiles ascend: under a causal mask the first ones carry
   // the most work.
   const int n_kv_tiles = (prm.Sk + kKv - 1) / kKv;
-  const int bh = blockIdx.x / n_kv_tiles;
+  const int bh = blockIdx.x / n_kv_tiles;         // (batch, K/V head)
   const int j = blockIdx.x - bh * n_kv_tiles;
-  const int h = bh % prm.H, b = bh / prm.H;
+  const int Hkv = kGqa ? prm.H / prm.G : prm.H;
+  const int h = bh % Hkv, b = bh / Hkv;           // h: the K/V head (= the query head without grouping)
   const int k0 = j * kKv;
   const int off = prm.Sk - prm.Sq;                // query q attends keys <= q + off
   const int n_q_tiles = (prm.Sq + kQt - 1) / kQt;
   const int i_begin = prm.causal ? max(0, k0 - off) / kQt : 0;
-  const int n_iter = n_q_tiles - i_begin;         // >= 1 for every key tile that holds a valid key
+  const int n_head_iter = n_q_tiles - i_begin;    // >= 1 for every key tile that holds a valid key
+  const int n_iter = kGqa ? n_head_iter * prm.G : n_head_iter;
+  // iteration it -> (query head, first query): the query tiles of the group's first head, then the next head's, ...
+  auto iter_head = [&](int it) { return kGqa ? h * prm.G + it / n_head_iter : h; };
+  auto iter_q0 = [&](int it) { return (i_begin + (kGqa ? it % n_head_iter : it)) * kQt; };
 
   if (warp == 4 && elect_one()) {
     tma_prefetch_desc(&tmap_q); tma_prefetch_desc(&tmap_k); tma_prefetch_desc(&tmap_v); tma_prefetch_desc(&tmap_do); tma_prefetch_desc(&tmap_dq);
@@ -129,14 +139,16 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
         tma_tile(&tmap_v, prm.swapped & 4u, kv_full, s_v + p * 8192, h * prm.hs_v + p * 64, k0, b);
       }
       for (int it = 0; it < n_iter; ++it) {
-        const int st = it % S::kStages, q0 = (i_begin + it) * kQt;
+        const int st = it % S::kStages, q0 = iter_q0(it);
+        const int hq = iter_head(it);
+        const int q_col = kGqa ? h * prm.gs_q + (hq - h * prm.G) * prm.hs_q : h * prm.hs_q;
         mbar_wait(q_empty(st), (((uint32_t)(it / S::kStages)) & 1u) ^ 1u);
         mbar_arrive_expect_tx(q_full(st), 2 * S::kQBytes + S::kStatBytes);
         for (int p = 0; p < kPanels; ++p) {
-          tma_tile(&tmap_q, prm.swapped & 1u, q_full(st), s_q + st * S::kQBytes + p * 8192, h * prm.hs_q + p * 64, q0, b);
-          tma_tile(&tmap_do, prm.swapped & 8u, q_full(st), s_do + st * S::kQBytes + p * 8192, h * prm.hs_do + p * 64, q0, b);
+          tma_tile(&tmap_q, prm.swapped & 1u, q_full(st), s_q + st * S::kQBytes + p * 8192, q_col + p * 64, q0, b);
+          tma_tile(&tmap_do, prm.swapped & 8u, q_full(st), s_do + st * S::kQBytes + p * 8192, hq * prm.hs_do + p * 64, q0, b);
         }
-        const size_t so = (size_t)bh * prm.Sq_pad + q0;
+        const size_t so = (kGqa ? (size_t)b * prm.H + hq : (size_t)bh) * prm.Sq_pad + q0;
         bulk_load_1d(s_stat + st * S::kStatBytes, prm.lse2 + so, kQt * 4, q_full(st));
         bulk_load_1d(s_stat + st * S::kStatBytes + kQt * 4, prm.delta + so, kQt * 4, q_full(st));
       }
@@ -148,7 +160,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
     const int k_row = (int)(warp * 16u + (lane >> 2));                // this thread's key rows inside the tile: k_row and k_row + 8
     const int col_in8 = (int)(lane & 3u) * 2;                         // ... and its query / channel pair inside every 8-column group
     const uint32_t pairs = ((uint32_t)prm.Sk + 1u) >> 1;
-    const uint32_t key = attn_rng_key(prm.seed, (uint32_t)bh);
+    uint32_t key = attn_rng_key(prm.seed, (uint32_t)(kGqa ? b * prm.H + h * prm.G : bh));
     const bool drop = prm.drop_thresh16 != 0;
     const float p_to_pdrop = prm.inv_keep / prm.scale;
     const bool leader = threadIdx.x == 0;
@@ -158,7 +170,9 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
     mbar_wait(kv_full, 0);
     for (int it = 0; it < n_iter; ++it) {
       const int st = it % S::kStages;
-      const int q0 = (i_begin + it) * kQt;
+      const int q0 = iter_q0(it);
+      const int hq = iter_head(it);
+      if (kGqa && it != 0 && q0 == i_begin * kQt) key = attn_rng_key(prm.seed, (uint32_t)(b * prm.H + hq));   // next head of the group
       const uint32_t sq = s_q + st * S::kQBytes, sdo = s_do + st * S::kQBytes;
       mbar_wait(q_full(st), ((uint32_t)(it / S::kStages)) & 1u);
       float s[kQt / 2], dp[kQt / 2];                                  // [4 g + e]: key k_row + 8 (e / 2), query 8 g + col_in8 + (e % 2)
@@ -248,7 +262,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
       asm volatile("bar.sync 1, 128;" ::: "memory");
       if (leader) {
         // rows of the 2-D [B*Sq, H*D] view; query rows past Sq of a ragged tile carry exact zeros (P = 0 there), rows past the tensor are dropped
-        tma_reduce_add_2d(&tmap_dq, s_dq, h * kHd, b * prm.Sq + q0);
+        tma_reduce_add_2d(&tmap_dq, s_dq, hq * kHd, b * prm.Sq + q0);
         tma_store_commit();
       }
     }
@@ -303,8 +317,9 @@ __global__ void attn_bwd_prep_kernel(const uint16_t* __restrict__ o, int64_t o_s
 }
 
 // ---- dq: fp32 accumulator -> 16-bit view
-template <bool kBf16>
-__global__ void attn_bwd_dq_convert_kernel(const float* __restrict__ acc, uint16_t* __restrict__ dq, int64_t sb, int64_t ss, int64_t sh, int B, int Sq, int H, int kHd) {
+template <bool kBf16, bool kGqa>    // kGqa: dq is a grouped view, head h at (h / G) * sg + (h % G) * sh
+__global__ void attn_bwd_dq_convert_kernel(const float* __restrict__ acc, uint16_t* __restrict__ dq, int64_t sb, int64_t ss, int64_t sh, int B, int Sq, int H, int kHd,
+                                           int G, int64_t sg) {
   const int64_t n8 = (int64_t)B * Sq * H * (kHd / 8);
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += (int64_t)gridDim.x * blockDim.x) {
     const int c = (int)(i % (kHd / 8));
@@ -315,7 +330,8 @@ __global__ void attn_bwd_dq_convert_kernel(const float* __restrict__ acc, uint16
     const float4 x = *reinterpret_cast<const float4*>(acc + i * 8), y = *reinterpret_cast<const float4*>(acc + i * 8 + 4);
     uint4 v;
     v.x = pack_16x2<kBf16>(x.x, x.y); v.y = pack_16x2<kBf16>(x.z, x.w); v.z = pack_16x2<kBf16>(y.x, y.y); v.w = pack_16x2<kBf16>(y.z, y.w);
-    *reinterpret_cast<uint4*>(dq + b * sb + s * ss + h * sh + c * 8) = v;
+    const int64_t ho = kGqa ? (h / G) * sg + (h % G) * sh : h * sh;
+    *reinterpret_cast<uint4*>(dq + b * sb + s * ss + ho + c * 8) = v;
   }
 }
 
@@ -323,17 +339,19 @@ bool view_ok(const AttnView& t) {
   return t.ptr != nullptr && (reinterpret_cast<uintptr_t>(t.ptr) % 16) == 0 && t.sb % 8 == 0 && t.ss % 8 == 0 && t.sh % 8 == 0;
 }
 
-bool make_map(CUtensorMap* m, const AttnView& t, int dtype, int B, int S, int H, int D, uint32_t box_rows, bool* swapped) {
-  const uint64_t inner = (uint64_t)(H - 1) * t.sh + D;
+// H: the view's heads.  G > 1: a grouped query view of H = Hkv * G heads (see AttnView)
+bool make_map(CUtensorMap* m, const AttnView& t, int dtype, int B, int S, int H, int D, uint32_t box_rows, bool* swapped, int G = 1) {
+  const uint64_t inner = G > 1 ? (uint64_t)(H / G - 1) * t.sg + (uint64_t)(G - 1) * t.sh + D : (uint64_t)(H - 1) * t.sh + D;
   return make_tmap_bshd(m, t.ptr, dtype, inner, (uint64_t)S, (uint64_t)B, (uint64_t)t.ss * 2, (uint64_t)t.sb * 2, 64, box_rows, swapped);
 }
 
 }  // namespace
 
-template <int kHd, bool kBf16>
+template <int kHd, bool kBf16, bool kGqa>
 static cudaError_t attention_bwd_impl(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, const AttnView& dout, const float* lse,
                                       const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int Sq,
-                                      int Sk, int H, float scale, bool causal, AttnDropout drop, cudaStream_t st) {
+                                      int Sk, int H, int Hkv, float scale, bool causal, AttnDropout drop, cudaStream_t st) {
+  const int G = H / Hkv;
   constexpr int D = kHd;
   constexpr int dt = kBf16 ? 1 : 0;
   using S = BwSmem<kHd>;
@@ -349,7 +367,7 @@ static cudaError_t attention_bwd_impl(const AttnView& q, const AttnView& k, cons
   }
   CUtensorMap tq, tk, tv, tdo, tdq;
   bool sq = false, sk = false, sv = false, sdo = false;
-  bool ok = make_map(&tq, q, dt, B, Sq, H, D, kQt, &sq) && make_map(&tk, k, dt, B, Sk, H, D, kKv, &sk) && make_map(&tv, v, dt, B, Sk, H, D, kKv, &sv) &&
+  bool ok = make_map(&tq, q, dt, B, Sq, H, D, kQt, &sq, G) && make_map(&tk, k, dt, B, Sk, Hkv, D, kKv, &sk) && make_map(&tv, v, dt, B, Sk, Hkv, D, kKv, &sv) &&
             make_map(&tdo, dout, dt, B, Sq, H, D, kQt, &sdo) &&
             make_tmap_2d_plain(&tdq, dq_acc, 3, (uint64_t)H * kHd, (uint64_t)B * Sq, (uint64_t)H * kHd * 4, kHd, kQt);
   if (!ok) return cudaErrorInvalidValue;
@@ -359,6 +377,7 @@ static cudaError_t attention_bwd_impl(const AttnView& q, const AttnView& k, cons
   prm.dv = BwOut{const_cast<void*>(dv.ptr), dv.sb, dv.ss, dv.sh};
   prm.B = B; prm.Sq = Sq; prm.Sk = Sk; prm.H = H; prm.Sq_pad = Sq_pad;
   prm.hs_q = (int)q.sh; prm.hs_k = (int)k.sh; prm.hs_v = (int)v.sh; prm.hs_do = (int)dout.sh;
+  prm.G = G; prm.gs_q = (int)q.sg;
   prm.swapped = (sq ? 1u : 0u) | (sk ? 2u : 0u) | (sv ? 4u : 0u) | (sdo ? 8u : 0u);
   prm.scale = scale; prm.scale_log2 = scale * 1.4426950408889634f;
   prm.causal = causal ? 1 : 0;
@@ -367,27 +386,30 @@ static cudaError_t attention_bwd_impl(const AttnView& q, const AttnView& k, cons
   prm.seed = drop.seed;
   static bool attr_set = false;
   if (!attr_set) {
-    if ((e = cudaFuncSetAttribute(attention_bwd_kernel<kHd, kBf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(attention_bwd_kernel<kHd, kBf16, kGqa>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal)) != cudaSuccess) return e;
     attr_set = true;
   }
   const int n_kv = (Sk + kKv - 1) / kKv;
-  attention_bwd_kernel<kHd, kBf16><<<(unsigned)(n_kv * B * H), kBwThreads, S::kTotal, st>>>(tq, tk, tv, tdo, tdq, prm);
+  attention_bwd_kernel<kHd, kBf16, kGqa><<<(unsigned)(n_kv * B * Hkv), kBwThreads, S::kTotal, st>>>(tq, tk, tv, tdo, tdq, prm);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  attn_bwd_dq_convert_kernel<kBf16><<<1184, 256, 0, st>>>(dq_acc, (uint16_t*)const_cast<void*>(dq.ptr), dq.sb, dq.ss, dq.sh, B, Sq, H, kHd);
+  attn_bwd_dq_convert_kernel<kBf16, kGqa><<<1184, 256, 0, st>>>(dq_acc, (uint16_t*)const_cast<void*>(dq.ptr), dq.sb, dq.ss, dq.sh, B, Sq, H, kHd, G, dq.sg);
   return cudaGetLastError();
 }
 
 cudaError_t attention_bwd(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, const AttnView& dout, const float* lse,
                           const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int Sq,
-                          int Sk, int H, int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st) {
+                          int Sk, int H, int Hkv, int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st) {
   if ((D != 64 && D != 128) || (dtype != 0 && dtype != 1) || B < 1 || Sq < 1 || Sk < 1 || (causal && Sk < Sq)) return cudaErrorInvalidValue;
+  if (H < 1 || Hkv < 1 || H % Hkv != 0 || (Hkv < H && (q.sg % 8 || dq.sg % 8))) return cudaErrorInvalidValue;
   for (const AttnView* t : {&q, &k, &v, &out, &dout, &dq, &dk, &dv}) if (!view_ok(*t)) return cudaErrorInvalidValue;
-  if (dtype == 1) {
-    if (D == 128) return attention_bwd_impl<128, true>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, Sq, Sk, H, scale, causal, drop, st);
-    return attention_bwd_impl<64, true>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, Sq, Sk, H, scale, causal, drop, st);
+#define PFX_BWD(HD, BF, GQA) attention_bwd_impl<HD, BF, GQA>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, Sq, Sk, H, Hkv, scale, causal, drop, st)
+  if (Hkv < H) {
+    if (dtype == 1) return D == 128 ? PFX_BWD(128, true, true) : PFX_BWD(64, true, true);
+    return D == 128 ? PFX_BWD(128, false, true) : PFX_BWD(64, false, true);
   }
-  if (D == 128) return attention_bwd_impl<128, false>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, Sq, Sk, H, scale, causal, drop, st);
-  return attention_bwd_impl<64, false>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, Sq, Sk, H, scale, causal, drop, st);
+  if (dtype == 1) return D == 128 ? PFX_BWD(128, true, false) : PFX_BWD(64, true, false);
+  return D == 128 ? PFX_BWD(128, false, false) : PFX_BWD(64, false, false);
+#undef PFX_BWD
 }
 
 }  // namespace pfx

@@ -8,6 +8,9 @@
 // shuffle reduction and each warp keeps a private online-softmax state (m, l, acc); the warps' partial states are merged through
 // shared memory at the end.  The op is a pure stream over the cache (2 * L * D * 2 bytes per head), so several keys are in flight
 // per warp.  Replaces the library SDPA call on the decode path (reference: hybrid_model.py:303-346 core attention with cache).
+//
+// Grouped-query attention (kGqa, a separate instantiation): the cache holds Hkv = H / G heads and query head h reads K/V head h / G.
+// The grid stays (query head, batch), so the G CTAs of a group are launch-order neighbours and their cache stream is served by L2.
 #include "pfx_common.cuh"
 #include "pfx_kernels.h"
 
@@ -20,10 +23,10 @@ constexpr int kDecWarps = 8;
 // D / 8 lanes share one key (16-byte loads of 8 channels each), so a warp works on 32 / (D / 8) keys at a time and keeps
 // kU such groups in flight: 8 (D = 128) or 16 (D = 64) keys = 4-8 KB per warp outstanding.  Every lane group carries its own
 // online-softmax state; all states of the CTA are merged through shared memory at the end.
-template <typename T, int D>
+template <typename T, int D, bool kGqa>
 __global__ void __launch_bounds__(kDecWarps * 32) attention_decode_kernel(const T* __restrict__ q, T* __restrict__ k, T* __restrict__ v,
                                                                            const T* __restrict__ mask, T* __restrict__ out, int L, int Lmax,
-                                                                           int H, float scale, const int64_t* __restrict__ write_idx) {
+                                                                           int H, float scale, const int64_t* __restrict__ write_idx, int G) {
   constexpr int kLanes = D / 8;               // lanes per key
   constexpr int kKW = 32 / kLanes;            // keys per warp step
   constexpr int kStates = kDecWarps * kKW;
@@ -33,25 +36,30 @@ __global__ void __launch_bounds__(kDecWarps * 32) attention_decode_kernel(const 
   const int h = blockIdx.x, b = blockIdx.y;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int sub = lane / kLanes, ch = (lane % kLanes) * 8;
+  const int Hkv = kGqa ? H / G : H, hk = kGqa ? h / G : h, g = h - hk * (kGqa ? G : 1);    // K/V head of this query head
   // packed mode (write_idx != null): q points at the fused QKV projection [B, 1, H, 3, D]; this CTA first appends its head's new
-  // key / value at cache position *write_idx (the cache write used to be two separate index_copy launches), then attends
+  // key / value at cache position *write_idx (the cache write used to be two separate index_copy launches), then attends.
+  // Grouped: qkv is [B, 1, Hkv, G + 2, D] (the group's G queries, then its key and value); the first CTA of a group appends, and
+  // since the CTAs of one launch are unordered, none of them reads that cache row: every one takes key *write_idx from qkv instead.
+  const T* qkv_row = kGqa && write_idx ? q + ((size_t)b * Hkv + hk) * (G + 2) * D : nullptr;
+  const int64_t new_pos = kGqa && write_idx ? write_idx[0] : -1;
   const int q_head_stride = write_idx ? 3 * D : D;
   if (write_idx != nullptr) {
     const int64_t pos = write_idx[0];
-    if (w < 2 && pos >= 0 && pos < Lmax) {
-      const T* src = q + ((size_t)b * H + h) * 3 * D + (1 + w) * D;
-      T* dst = (w == 0 ? k : v) + ((size_t)b * Lmax + pos) * H * D + (size_t)h * D;
+    if (w < 2 && pos >= 0 && pos < Lmax && g == 0) {
+      const T* src = kGqa ? qkv_row + (G + w) * D : q + ((size_t)b * H + h) * 3 * D + (1 + w) * D;
+      T* dst = (w == 0 ? k : v) + ((size_t)b * Lmax + pos) * Hkv * D + (size_t)hk * D;
       for (int i = lane; i < D; i += 32) dst[i] = src[i];
     }
-    __syncthreads();
+    if (!kGqa) __syncthreads();
   }
   float qv[8];
-  unpack8<T>(*reinterpret_cast<const uint4*>(q + ((size_t)b * H + h) * q_head_stride + ch), qv);
+  unpack8<T>(*reinterpret_cast<const uint4*>(kGqa && write_idx ? qkv_row + g * D + ch : q + ((size_t)b * H + h) * q_head_stride + ch), qv);
 #pragma unroll
   for (int i = 0; i < 8; ++i) qv[i] *= scale;
-  const size_t row_stride = (size_t)H * D;
-  const T* kb = k + (size_t)b * Lmax * row_stride + (size_t)h * D + ch;
-  const T* vb = v + (size_t)b * Lmax * row_stride + (size_t)h * D + ch;
+  const size_t row_stride = (size_t)Hkv * D;
+  const T* kb = k + (size_t)b * Lmax * row_stride + (size_t)hk * D + ch;
+  const T* vb = v + (size_t)b * Lmax * row_stride + (size_t)hk * D + ch;
   const T* mb = mask ? mask + (size_t)b * Lmax : nullptr;
   float m = -INFINITY, l = 0.f, acc[8];
 #pragma unroll
@@ -61,7 +69,10 @@ __global__ void __launch_bounds__(kDecWarps * 32) attention_decode_kernel(const 
 #pragma unroll
     for (int u = 0; u < kU; ++u) {
       const int t = t0 + u * kKW + sub;
-      if (t < L) {
+      if (kGqa && t == new_pos) {
+        rk[u] = *reinterpret_cast<const uint4*>(qkv_row + G * D + ch);
+        rv[u] = *reinterpret_cast<const uint4*>(qkv_row + (G + 1) * D + ch);
+      } else if (t < L) {
         rk[u] = ld_stream(reinterpret_cast<const uint4*>(kb + (size_t)t * row_stride));
         rv[u] = ld_stream(reinterpret_cast<const uint4*>(vb + (size_t)t * row_stride));
       }
@@ -113,14 +124,18 @@ __global__ void __launch_bounds__(kDecWarps * 32) attention_decode_kernel(const 
 }  // namespace
 
 cudaError_t attention_decode(const void* q, void* k, void* v, const void* mask, void* out, int B, int H, int D, int L, int Lmax,
-                             float scale, int dtype, cudaStream_t st, const int64_t* write_idx) {
+                             float scale, int dtype, cudaStream_t st, const int64_t* write_idx, int Hkv) {
   if (!B || !H) return cudaSuccess;
-  if ((D != 64 && D != 128) || L < 1 || L > Lmax) return cudaErrorInvalidValue;
+  if (Hkv == 0) Hkv = H;
+  if ((D != 64 && D != 128) || L < 1 || L > Lmax || Hkv < 1 || H % Hkv != 0) return cudaErrorInvalidValue;
   const dim3 grid(H, B), block(kDecWarps * 32);
-#define PFX_AD(T, P) attention_decode_kernel<T, P><<<grid, block, 0, st>>>((const T*)q, (T*)k, (T*)v, (const T*)mask, (T*)out, L, Lmax, H, scale, write_idx)
-  if (dtype == 1) { if (D == 128) PFX_AD(__nv_bfloat16, 128); else PFX_AD(__nv_bfloat16, 64); }
-  else if (dtype == 0) { if (D == 128) PFX_AD(__half, 128); else PFX_AD(__half, 64); }
+  const int G = H / Hkv;
+#define PFX_AD(T, P, GQA) attention_decode_kernel<T, P, GQA><<<grid, block, 0, st>>>((const T*)q, (T*)k, (T*)v, (const T*)mask, (T*)out, L, Lmax, H, scale, write_idx, G)
+#define PFX_AD_D(T, GQA) do { if (D == 128) PFX_AD(T, 128, GQA); else PFX_AD(T, 64, GQA); } while (0)
+  if (dtype == 1) { if (G > 1) PFX_AD_D(__nv_bfloat16, true); else PFX_AD_D(__nv_bfloat16, false); }
+  else if (dtype == 0) { if (G > 1) PFX_AD_D(__half, true); else PFX_AD_D(__half, false); }
   else return cudaErrorInvalidValue;
+#undef PFX_AD_D
 #undef PFX_AD
   return cudaGetLastError();
 }

@@ -52,11 +52,16 @@ __device__ __forceinline__ void tma3(const CUtensorMap* m, bool swapped, uint32_
   if (swapped) tma_load_3d(m, bar, dst, col, b, s); else tma_load_3d(m, bar, dst, col, s, b);
 }
 
-template <int kD, bool kCausal, bool kBf16>   // kBf16: bf16 operands and output, otherwise fp16
+// kBf16: bf16 operands and output, otherwise fp16.  kGqa: G = H / Hkv > 1 query heads share one K/V head (a separate instantiation, so
+// the multi-head kernels are compiled exactly as without it); query head h loads Q at column (h / G) * gs_q + (h % G) * hs_q and K / V
+// of head h / G.  The work order keeps the heads of one batch adjacent, so the G query heads of a group stream the same K / V tiles
+// at about the same time and share them through L2.
+template <int kD, bool kCausal, bool kBf16, bool kGqa>
 __global__ void __launch_bounds__(kFaThreads, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v,
                      uint16_t* __restrict__ out, int64_t o_sb, int64_t o_ss, int64_t o_sh, float* __restrict__ lse, int B, int Sq, int Sk, int H,
-                     float scale_log2, int hs_q, int hs_k, int hs_v, uint32_t swapped, uint32_t drop_thresh16, float inv_keep, uint64_t seed) {
+                     float scale_log2, int hs_q, int hs_k, int hs_v, uint32_t swapped, uint32_t drop_thresh16, float inv_keep, uint64_t seed,
+                     int G, int gs_q) {
   using S = FaSmem<kD>;
   constexpr int kPanels = kD / 64;                 // 64-element (128-byte) column panels of a D-wide tile
   extern __shared__ uint8_t smem_raw[];
@@ -95,19 +100,21 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
       for (int w = blockIdx.x; w < n_items; w += gridDim.x, ++it) {
         const int q_tile = item_tile(w), hb = w % hb_count, h = hb % H, b = hb / H;
         const int n_kv = tile_n_kv(q_tile);
+        const int q_col = kGqa ? (h / G) * gs_q + (h % G) * hs_q : h * hs_q;
+        const int hk = kGqa ? h / G : h;
         mbar_wait(q_empty, ((uint32_t)it & 1u) ^ 1u);
         mbar_arrive_expect_tx(q_full, S::kQBytes);
-        for (int p = 0; p < kPanels; ++p) tma3(&tmap_q, swapped & 1u, q_full, smem_q + p * (kFaQ * 128), h * hs_q + p * 64, q_tile * kFaQ, b);
+        for (int p = 0; p < kPanels; ++p) tma3(&tmap_q, swapped & 1u, q_full, smem_q + p * (kFaQ * 128), q_col + p * 64, q_tile * kFaQ, b);
         for (int j = 0; j < n_kv; ++j, ++t) {
           const int stage = t & 1;
           mbar_wait(kv_empty(stage), ((t >> 1) & 1u) ^ 1u);
           const uint32_t sk = smem_kv + stage * S::kStageBytes, sv = sk + S::kKBytes;
           mbar_arrive_expect_tx(kv_full(stage), S::kStageBytes);
           const int key0 = j * kFaKv;
-          for (int p = 0; p < kPanels; ++p) tma3(&tmap_k, swapped & 2u, kv_full(stage), sk + p * (kFaKv * 128), h * hs_k + p * 64, key0, b);
+          for (int p = 0; p < kPanels; ++p) tma3(&tmap_k, swapped & 2u, kv_full(stage), sk + p * (kFaKv * 128), hk * hs_k + p * 64, key0, b);
           for (int kb = 0; kb < 2; ++kb)            // V as the MN-major B operand: [64 keys x 64 channels] boxes, channel chunks 8 KB apart
             for (int nc = 0; nc < kPanels; ++nc)
-              tma3(&tmap_v, swapped & 4u, kv_full(stage), sv + (kb * kPanels + nc) * 8192, h * hs_v + nc * 64, key0 + kb * 64, b);
+              tma3(&tmap_v, swapped & 4u, kv_full(stage), sv + (kb * kPanels + nc) * 8192, hk * hs_v + nc * 64, key0 + kb * 64, b);
         }
       }
     }
@@ -219,19 +226,22 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
   }
 }
 
-template <int kD, bool kCausal, bool kBf16>
-cudaError_t launch_fa(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H, float scale,
-                      AttnDropout drop, cudaStream_t st) {
+template <int kD, bool kCausal, bool kBf16, bool kGqa>
+cudaError_t launch_fa(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H, int Hkv,
+                      float scale, AttnDropout drop, cudaStream_t st) {
   using S = FaSmem<kD>;
   CUtensorMap tq, tk, tv;
   bool sq = false, sk = false, sv = false;
-  auto inner = [&](const AttnView& t) { return (uint64_t)(H - 1) * t.sh + kD; };
+  const int G = H / Hkv;
+  // the maps' inner extent reaches the furthest column a head reads
+  const uint64_t inner_q = kGqa ? (uint64_t)(Hkv - 1) * q.sg + (uint64_t)(G - 1) * q.sh + kD : (uint64_t)(H - 1) * q.sh + kD;
+  auto inner = [&](const AttnView& t) { return (uint64_t)(Hkv - 1) * t.sh + kD; };
   constexpr int dt = kBf16 ? 1 : 0;
-  bool ok = make_tmap_bshd(&tq, q.ptr, dt, inner(q), Sq, B, (uint64_t)q.ss * 2, (uint64_t)q.sb * 2, 64, kFaQ, &sq);
+  bool ok = make_tmap_bshd(&tq, q.ptr, dt, inner_q, Sq, B, (uint64_t)q.ss * 2, (uint64_t)q.sb * 2, 64, kFaQ, &sq);
   ok &= make_tmap_bshd(&tk, k.ptr, dt, inner(k), Sk, B, (uint64_t)k.ss * 2, (uint64_t)k.sb * 2, 64, kFaKv, &sk);
   ok &= make_tmap_bshd(&tv, v.ptr, dt, inner(v), Sk, B, (uint64_t)v.ss * 2, (uint64_t)v.sb * 2, 64, 64, &sv);
   if (!ok) return cudaErrorInvalidValue;
-  auto kern = attention_fwd_kernel<kD, kCausal, kBf16>;
+  auto kern = attention_fwd_kernel<kD, kCausal, kBf16, kGqa>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal);
@@ -249,33 +259,39 @@ cudaError_t launch_fa(const AttnView& q, const AttnView& k, const AttnView& v, c
   const float inv_keep = drop.p > 0.f ? 1.f / (1.f - drop.p) : 1.f;
   const uint32_t swapped = (sq ? 1u : 0u) | (sk ? 2u : 0u) | (sv ? 4u : 0u);
   kern<<<grid, kFaThreads, S::kTotal, st>>>(tq, tk, tv, (uint16_t*)const_cast<void*>(out.ptr), out.sb, out.ss, out.sh, lse, B, Sq, Sk, H,
-                                            scale * 1.4426950408889634f, (int)q.sh, (int)k.sh, (int)v.sh, swapped, thresh, inv_keep, drop.seed);
+                                            scale * 1.4426950408889634f, (int)q.sh, (int)k.sh, (int)v.sh, swapped, thresh, inv_keep, drop.seed, G, (int)q.sg);
   return cudaGetLastError();
 }
 
-template <bool kBf16>
+template <bool kBf16, bool kGqa>
 cudaError_t launch_fa_dt(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H,
-                         int D, float scale, bool causal, AttnDropout drop, cudaStream_t st) {
-  if (D == 128) return causal ? launch_fa<128, true, kBf16>(q, k, v, out, lse, B, Sq, Sk, H, scale, drop, st) : launch_fa<128, false, kBf16>(q, k, v, out, lse, B, Sq, Sk, H, scale, drop, st);
-  return causal ? launch_fa<64, true, kBf16>(q, k, v, out, lse, B, Sq, Sk, H, scale, drop, st) : launch_fa<64, false, kBf16>(q, k, v, out, lse, B, Sq, Sk, H, scale, drop, st);
+                         int Hkv, int D, float scale, bool causal, AttnDropout drop, cudaStream_t st) {
+  if (D == 128) return causal ? launch_fa<128, true, kBf16, kGqa>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, scale, drop, st)
+                              : launch_fa<128, false, kBf16, kGqa>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, scale, drop, st);
+  return causal ? launch_fa<64, true, kBf16, kGqa>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, scale, drop, st)
+                : launch_fa<64, false, kBf16, kGqa>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, scale, drop, st);
 }
 
 }  // namespace
 
 cudaError_t attention_fwd_v2(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H,
-                             int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st) {
+                             int Hkv, int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st) {
   if ((D != 64 && D != 128) || (dtype != 0 && dtype != 1) || B < 1 || Sq < 1 || Sk < 1 || (causal && Sk < Sq)) return cudaErrorInvalidValue;
+  if (H < 1 || Hkv < 1 || H % Hkv != 0 || (Hkv < H && q.sg % 8)) return cudaErrorInvalidValue;
   for (const AttnView* t : {&q, &k, &v, &out})
     if (t->ptr == nullptr || (reinterpret_cast<uintptr_t>(t->ptr) % 16) || t->sb % 8 || t->ss % 8 || t->sh % 8) return cudaErrorInvalidValue;
-  return dtype == 1 ? launch_fa_dt<true>(q, k, v, out, lse, B, Sq, Sk, H, D, scale, causal, drop, st)
-                    : launch_fa_dt<false>(q, k, v, out, lse, B, Sq, Sk, H, D, scale, causal, drop, st);
+  if (Hkv < H)
+    return dtype == 1 ? launch_fa_dt<true, true>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, D, scale, causal, drop, st)
+                      : launch_fa_dt<false, true>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, D, scale, causal, drop, st);
+  return dtype == 1 ? launch_fa_dt<true, false>(q, k, v, out, lse, B, Sq, Sk, H, H, D, scale, causal, drop, st)
+                    : launch_fa_dt<false, false>(q, k, v, out, lse, B, Sq, Sk, H, H, D, scale, causal, drop, st);
 }
 
 cudaError_t attention_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Sq, int Sk, int H, int D, float scale,
                           bool causal, cudaStream_t st) {
   const int64_t hd = (int64_t)H * D;
   const AttnView vq{q, (int64_t)Sq * hd, hd, D}, vk{k, (int64_t)Sk * hd, hd, D}, vv{v, (int64_t)Sk * hd, hd, D}, vo{out, (int64_t)Sq * hd, hd, D};
-  return attention_fwd_v2(vq, vk, vv, vo, lse, B, Sq, Sk, H, D, scale, causal, AttnDropout{0.f, 0}, 1, st);
+  return attention_fwd_v2(vq, vk, vv, vo, lse, B, Sq, Sk, H, H, D, scale, causal, AttnDropout{0.f, 0}, 1, st);
 }
 
 }  // namespace pfx

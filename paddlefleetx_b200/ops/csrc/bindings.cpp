@@ -630,10 +630,12 @@ at::Tensor gemm_smallm(const at::Tensor& x, const at::Tensor& w, c10::optional<a
 }
 
 at::Tensor attention_decode(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v, c10::optional<at::Tensor> mask, int64_t L, double scale) {
-  // q [B,1,H,D]; k, v [B,Lmax,H,D] (contiguous cache); mask additive [B,Lmax] in the same dtype, or none
+  // q [B,1,H,D]; k, v [B,Lmax,Hkv,D] (contiguous cache, H % Hkv == 0); mask additive [B,Lmax] in the same dtype, or none
   PFX_CHECK_CUDA_CONTIG(q); PFX_CHECK_CUDA_CONTIG(k); PFX_CHECK_CUDA_CONTIG(v);
-  TORCH_CHECK(q.dim() == 4 && q.size(1) == 1 && k.dim() == 4 && k.sizes() == v.sizes() && k.size(0) == q.size(0) && k.size(2) == q.size(2) &&
-              k.size(3) == q.size(3) && k.scalar_type() == q.scalar_type(), "attention_decode: shape mismatch");
+  TORCH_CHECK(q.dim() == 4 && q.size(1) == 1 && k.dim() == 4 && k.sizes() == v.sizes() && k.size(0) == q.size(0) &&
+              k.size(3) == q.size(3) && k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type(), "attention_decode: shape mismatch");
+  TORCH_CHECK(k.size(2) >= 1 && q.size(2) % k.size(2) == 0, "attention_decode: q has ", q.size(2), " heads, which is not a multiple of the ",
+              k.size(2), " cache heads");
   const c10::cuda::CUDAGuard guard(q.device());
   const void* mp = nullptr;
   at::Tensor mc;
@@ -644,7 +646,7 @@ at::Tensor attention_decode(const at::Tensor& q, const at::Tensor& k, const at::
   }
   auto out = at::empty_like(q);
   PFX_CUDA_CHECK(pfx::attention_decode(q.data_ptr(), k.data_ptr(), v.data_ptr(), mp, out.data_ptr(), (int)q.size(0), (int)q.size(2), (int)q.size(3),
-                                       (int)L, (int)k.size(1), (float)scale, dtype_code(q), cur_stream()));
+                                       (int)L, (int)k.size(1), (float)scale, dtype_code(q), cur_stream(), nullptr, (int)k.size(2)));
   return out;
 }
 
@@ -700,17 +702,45 @@ static pfx::AttnView attn_view(const at::Tensor& t, const char* name) {
   return pfx::AttnView{t.data_ptr(), t.stride(0), t.stride(1), t.stride(2)};
 }
 
+// Query heads of q (or dq): [B,S,H,D], or [B,S,Hkv,G,D] for the query part of a packed [B,S,Hkv,G+2,D] grouped projection output.
+static int64_t attn_q_heads(const at::Tensor& t) { return t.dim() == 5 ? t.size(2) * t.size(3) : t.size(2); }
+
+// The view of q / dq when k / v have Hkv heads: a [B,S,H,D] view (group stride G * head stride) or a [B,S,Hkv,G,D] view.
+static pfx::AttnView attn_qview(const at::Tensor& t, const char* name, int64_t Hkv) {
+  if (t.dim() != 5) {
+    pfx::AttnView v = attn_view(t, name);
+    v.sg = (t.size(2) / Hkv) * t.stride(2);
+    return v;
+  }
+  TORCH_CHECK(t.is_cuda() && is_16bit(t) && t.stride(4) == 1, name, ": [B,S,Hkv,G,D] bf16 or fp16 CUDA view with contiguous D expected");
+  TORCH_CHECK(t.size(2) == Hkv, name, ": a [B,S,Hkv,G,D] view needs one group per K/V head (", t.size(2), " groups, ", Hkv, " K/V heads)");
+  TORCH_CHECK(t.stride(0) % 8 == 0 && t.stride(1) % 8 == 0 && t.stride(2) % 8 == 0 && t.stride(3) % 8 == 0 &&
+              (reinterpret_cast<uintptr_t>(t.data_ptr()) % 16) == 0, name, ": strides must be multiples of 8 elements and the base 16-byte aligned");
+  return pfx::AttnView{t.data_ptr(), t.stride(0), t.stride(1), t.stride(3), t.stride(2)};
+}
+
+// k / v heads against the query heads of q: returns Hkv (H % Hkv == 0 is required)
+static int64_t attn_kv_heads(const at::Tensor& q, const at::Tensor& k, const char* fn) {
+  TORCH_CHECK(q.dim() == 4 || q.dim() == 5, fn, ": q must be [B,S,H,D] or [B,S,Hkv,G,D]");
+  TORCH_CHECK(k.dim() == 4, fn, ": k must be [B,S,Hkv,D]");
+  const int64_t H = attn_q_heads(q), Hkv = k.size(2);
+  TORCH_CHECK(Hkv >= 1 && H % Hkv == 0, fn, ": q has ", H, " heads, which is not a multiple of the ", Hkv, " K/V heads");
+  return Hkv;
+}
+
 // Flash attention forward on [B,S,H,D] bf16 or fp16 views (no copies for packed-QKV slices / sequence-major storage); optional dropout keyed by `seed`.
+// Grouped-query attention: k / v may have Hkv heads with H % Hkv == 0, and q may be the [B,S,Hkv,G,D] query part of a packed projection.
 std::vector<at::Tensor> attention_fwd_v2(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v, bool causal, double scale, double dropout_p,
                                          int64_t seed) {
-  TORCH_CHECK(q.dim() == 4 && k.dim() == 4 && k.sizes() == v.sizes() && q.size(0) == k.size(0) && q.size(2) == k.size(2) && q.size(3) == k.size(3),
-              "attention_fwd_v2: shape mismatch");
+  const int64_t Hkv = attn_kv_heads(q, k, "attention_fwd_v2");
+  const int64_t H = attn_q_heads(q), D = q.size(q.dim() - 1);
+  TORCH_CHECK(k.sizes() == v.sizes() && q.size(0) == k.size(0) && D == k.size(3), "attention_fwd_v2: shape mismatch");
   TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type(), "attention_fwd_v2: q, k, v must have one dtype");
   const c10::cuda::CUDAGuard guard(q.device());
-  auto out = at::empty({q.size(0), q.size(1), q.size(2), q.size(3)}, q.options());
-  auto lse = at::empty({q.size(0), q.size(2), q.size(1)}, q.options().dtype(at::kFloat));
-  PFX_CUDA_CHECK(pfx::attention_fwd_v2(attn_view(q, "q"), attn_view(k, "k"), attn_view(v, "v"), attn_view(out, "out"), lse.data_ptr<float>(),
-                                       (int)q.size(0), (int)q.size(1), (int)k.size(1), (int)q.size(2), (int)q.size(3), (float)scale, causal,
+  auto out = at::empty({q.size(0), q.size(1), H, D}, q.options());
+  auto lse = at::empty({q.size(0), H, q.size(1)}, q.options().dtype(at::kFloat));
+  PFX_CUDA_CHECK(pfx::attention_fwd_v2(attn_qview(q, "q", Hkv), attn_view(k, "k"), attn_view(v, "v"), attn_view(out, "out"), lse.data_ptr<float>(),
+                                       (int)q.size(0), (int)q.size(1), (int)k.size(1), (int)H, (int)Hkv, (int)D, (float)scale, causal,
                                        pfx::AttnDropout{(float)dropout_p, (uint64_t)seed}, dtype_code(q), cur_stream()));
   return {out, lse};
 }
@@ -718,29 +748,37 @@ std::vector<at::Tensor> attention_fwd_v2(const at::Tensor& q, const at::Tensor& 
 // Flash attention backward (head_dim 64 or 128, bf16 or fp16): writes dq / dk / dv into the given (possibly strided) views.
 void attention_bwd(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v, const at::Tensor& out, const at::Tensor& dout, const at::Tensor& lse,
                    at::Tensor& dq, at::Tensor& dk, at::Tensor& dv, bool causal, double scale, double dropout_p, int64_t seed) {
-  TORCH_CHECK(q.dim() == 4 && k.sizes() == v.sizes() && q.sizes() == out.sizes() && q.sizes() == dout.sizes() && q.sizes() == dq.sizes() &&
-              k.sizes() == dk.sizes() && k.sizes() == dv.sizes() && (q.size(3) == 128 || q.size(3) == 64), "attention_bwd: shape mismatch (head_dim must be 64 or 128)");
-  TORCH_CHECK(lse.is_cuda() && lse.is_contiguous() && lse.scalar_type() == at::kFloat && lse.numel() == q.size(0) * q.size(1) * q.size(2), "attention_bwd: lse");
+  const int64_t Hkv = attn_kv_heads(q, k, "attention_bwd");
+  const int64_t H = attn_q_heads(q), D = q.size(q.dim() - 1);
+  TORCH_CHECK(D == 128 || D == 64, "attention_bwd: head_dim must be 64 or 128");
+  TORCH_CHECK(k.sizes() == v.sizes() && q.size(0) == k.size(0) && D == k.size(3), "attention_bwd: k / v shape mismatch");
+  TORCH_CHECK(k.sizes() == dk.sizes() && k.sizes() == dv.sizes(), "attention_bwd: dk / dv must have the shape of k");
+  TORCH_CHECK(q.sizes() == dq.sizes(), "attention_bwd: dq must have the shape of q");
+  const std::vector<int64_t> o_shape{q.size(0), q.size(1), H, D};
+  TORCH_CHECK(out.sizes() == at::IntArrayRef(o_shape) && dout.sizes() == at::IntArrayRef(o_shape), "attention_bwd: out / dout must be [B,Sq,H,D]");
+  TORCH_CHECK(lse.is_cuda() && lse.is_contiguous() && lse.scalar_type() == at::kFloat && lse.numel() == q.size(0) * q.size(1) * H, "attention_bwd: lse");
   for (const at::Tensor* t : std::initializer_list<const at::Tensor*>{&k, &v, &out, &dout, &dq, &dk, &dv})
     TORCH_CHECK(t->scalar_type() == q.scalar_type(), "attention_bwd: q, k, v, out, dout and the gradients must have one dtype");
   const c10::cuda::CUDAGuard guard(q.device());
-  const int64_t B = q.size(0), Sq = q.size(1), Sk = k.size(1), H = q.size(2), D = q.size(3);
+  const int64_t B = q.size(0), Sq = q.size(1), Sk = k.size(1);
   const int64_t sq_pad = (Sq + 63) / 64 * 64;
   auto f32 = q.options().dtype(at::kFloat);
   auto dq_acc = at::empty({B, Sq, H, D}, f32);
   auto stats = at::empty({2, B * H * sq_pad}, f32);
-  PFX_CUDA_CHECK(pfx::attention_bwd(attn_view(q, "q"), attn_view(k, "k"), attn_view(v, "v"), attn_view(out, "out"), attn_view(dout, "dout"),
-                                    lse.data_ptr<float>(), attn_view(dq, "dq"), attn_view(dk, "dk"), attn_view(dv, "dv"), dq_acc.data_ptr<float>(),
-                                    stats[0].data_ptr<float>(), stats[1].data_ptr<float>(), (int)B, (int)Sq, (int)Sk, (int)H, (int)D, (float)scale,
+  PFX_CUDA_CHECK(pfx::attention_bwd(attn_qview(q, "q", Hkv), attn_view(k, "k"), attn_view(v, "v"), attn_view(out, "out"), attn_view(dout, "dout"),
+                                    lse.data_ptr<float>(), attn_qview(dq, "dq", Hkv), attn_view(dk, "dk"), attn_view(dv, "dv"), dq_acc.data_ptr<float>(),
+                                    stats[0].data_ptr<float>(), stats[1].data_ptr<float>(), (int)B, (int)Sq, (int)Sk, (int)H, (int)Hkv, (int)D, (float)scale,
                                     causal, pfx::AttnDropout{(float)dropout_p, (uint64_t)seed}, dtype_code(q), cur_stream()));
 }
 
 at::Tensor attention_decode_packed(const at::Tensor& qkv, at::Tensor& k, at::Tensor& v, c10::optional<at::Tensor> mask, const at::Tensor& write_idx,
                                    double scale) {
-  // qkv [B,1,H,3,D] (fused projection output); appends this step's K/V at cache position write_idx[0] and attends over the whole cache
+  // qkv [B,1,Hkv,G+2,D] (fused projection output: per K/V head its G queries, key and value; G = 1 is [B,1,H,3,D]); appends this step's
+  // K/V at cache position write_idx[0] and attends over the whole cache [B,Lmax,Hkv,D]
   PFX_CHECK_CUDA_CONTIG(qkv); PFX_CHECK_CUDA_CONTIG(k); PFX_CHECK_CUDA_CONTIG(v);
-  TORCH_CHECK(qkv.dim() == 5 && qkv.size(1) == 1 && qkv.size(3) == 3 && k.dim() == 4 && k.sizes() == v.sizes() && k.size(0) == qkv.size(0) &&
-              k.size(2) == qkv.size(2) && k.size(3) == qkv.size(4) && k.scalar_type() == qkv.scalar_type(), "attention_decode_packed: shape mismatch");
+  TORCH_CHECK(qkv.dim() == 5 && qkv.size(1) == 1 && qkv.size(3) >= 3 && k.dim() == 4 && k.sizes() == v.sizes() && k.size(0) == qkv.size(0) &&
+              k.size(2) == qkv.size(2) && k.size(3) == qkv.size(4) && k.scalar_type() == qkv.scalar_type() && v.scalar_type() == qkv.scalar_type(),
+              "attention_decode_packed: shape mismatch (qkv [B,1,Hkv,G+2,D], caches [B,Lmax,Hkv,D])");
   TORCH_CHECK(write_idx.is_cuda() && write_idx.scalar_type() == at::kLong && write_idx.numel() == 1, "attention_decode_packed: write_idx");
   const c10::cuda::CUDAGuard guard(qkv.device());
   const void* mp = nullptr;
@@ -750,10 +788,11 @@ at::Tensor attention_decode_packed(const at::Tensor& qkv, at::Tensor& k, at::Ten
     TORCH_CHECK(mc.size(1) == k.size(1), "attention_decode_packed: mask must cover the whole cache");
     mp = mc.data_ptr();
   }
-  auto out = at::empty({qkv.size(0), 1, qkv.size(2), qkv.size(4)}, qkv.options());
-  PFX_CUDA_CHECK(pfx::attention_decode(qkv.data_ptr(), k.data_ptr(), v.data_ptr(), mp, out.data_ptr(), (int)qkv.size(0), (int)qkv.size(2),
+  const int64_t Hkv = qkv.size(2), H = Hkv * (qkv.size(3) - 2);
+  auto out = at::empty({qkv.size(0), 1, H, qkv.size(4)}, qkv.options());
+  PFX_CUDA_CHECK(pfx::attention_decode(qkv.data_ptr(), k.data_ptr(), v.data_ptr(), mp, out.data_ptr(), (int)qkv.size(0), (int)H,
                                        (int)qkv.size(4), (int)k.size(1), (int)k.size(1), (float)scale, dtype_code(qkv), cur_stream(),
-                                       write_idx.data_ptr<int64_t>()));
+                                       write_idx.data_ptr<int64_t>(), (int)Hkv));
   return out;
 }
 

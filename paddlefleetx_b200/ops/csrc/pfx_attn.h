@@ -7,9 +7,14 @@ namespace pfx {
 
 // A [B, S, H, D] 16-bit view with D contiguous; strides in elements.  Covers contiguous tensors, the q / k / v slices of a packed
 // [B, S, H, 3, D] projection output and sequence-major ([S, B, ...]) storage without any copy.
+//
+// Grouped-query attention (Hkv K/V heads, G = H / Hkv query heads per K/V head): k / v / dk / dv have Hkv heads; q and dq are
+// addressed per query head h as (h / G) * sg + (h % G) * sh, which also covers the q slice of a packed [B, S, Hkv, G + 2, D]
+// projection output (no uniform head stride there).  sg is read only when G > 1; a uniform view has sg = G * sh.
 struct AttnView {
   const void* ptr;
   int64_t sb, ss, sh;
+  int64_t sg = 0;
 };
 
 struct AttnDropout {
@@ -19,14 +24,17 @@ struct AttnDropout {
 
 // O = softmax(scale * Q K^T + causal) (dropout) V;  lse = row-wise log-sum-exp (natural log) [B, H, Sq] fp32.
 // dtype: 1 = bf16, 0 = fp16, for every view of the call (the flash kernels are compiled for both).
+// H query heads, Hkv K/V heads (H % Hkv == 0); query head h reads K/V head h / (H / Hkv).  LSE, out and the dropout key stay per query
+// head, so a grouped call drops the same elements as an H-head call with K/V repeated per group.
 cudaError_t attention_fwd_v2(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H,
-                             int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st);
+                             int Hkv, int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st);
 
 // Backward.  Workspace: dq_acc fp32 [B, Sq, H, D] (zeroed by the call), lse2 / delta fp32 [B, H, round_up(Sq, 64)].
 // dq / dk / dv may be strided views (e.g. slices of one packed [B, S, H, 3, D] gradient buffer).  D is 64 or 128; dtype as above.
+// With Hkv < H one CTA per (batch, K/V head, key tile) walks the query tiles of every head of the group, so dk / dv are written once.
 cudaError_t attention_bwd(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, const AttnView& dout, const float* lse,
                           const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int Sq,
-                          int Sk, int H, int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st);
+                          int Sk, int H, int Hkv, int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st);
 
 // Evoformer gated attention (head width 32, H even): softmax(scale QK^T + mask_bias[g, k] + pair_bias[g / groups_per_pair, h, q, k]) V * sigmoid(gate).
 // q / out / gate [G, Sq, H, 32], k / v [G, Sk, H, 32] bf16 contiguous; mask_bias fp32 [G, Sk]; pair_bias bf16; lse fp32 [G, H, Sq].

@@ -70,9 +70,9 @@ cudaError_t gemm_smallm(const void* x, const void* w, const void* bias, void* y,
 cudaError_t attention_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Sq, int Sk, int H, int D, float scale,
                           bool causal, cudaStream_t st);
 
-// attention_decode.cu — single-query attention over the static KV cache
+// attention_decode.cu — single-query attention over the static KV cache.  H query heads, Hkv cache heads (0 = H; H % Hkv == 0).
 cudaError_t attention_decode(const void* q, void* k, void* v, const void* mask, void* out, int B, int H, int D, int L, int Lmax,
-                             float scale, int dtype, cudaStream_t st, const int64_t* write_idx = nullptr);
+                             float scale, int dtype, cudaStream_t st, const int64_t* write_idx = nullptr, int Hkv = 0);
 
 
 // embedding.cu — fused word (+ position) look-up; deterministic sorted scatter-add gradient (workspace: next_pow2(tokens) 64-bit keys)

@@ -295,22 +295,28 @@ def gemv_fused(x: torch.Tensor, weight: torch.Tensor, bias=None, ln=None, residu
 
 def attention_decode_packed(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, additive_mask: torch.Tensor, write_idx: torch.Tensor,
                             scale: float) -> torch.Tensor:
-    """``qkv`` [B,1,H,3,D]: append this token's K/V at ``write_idx`` and attend over the whole static cache (one kernel)."""
+    """``qkv`` [B,1,H,3,D], or [B,1,Hkv,G+2,D] with grouped K/V heads (per K/V head: its G queries, key, value): append this token's
+    K/V at ``write_idx`` and attend over the whole static cache [B,Lmax,Hkv,D] (one kernel)."""
     if qkv.is_cuda and _native.available():
         _count()
         return _native.require().attention_decode_packed(qkv.contiguous(), k_cache, v_cache, additive_mask, write_idx, float(scale))
-    q, k, v = qkv.unbind(3)
+    g = qkv.shape[3] - 2
+    q, k, v = qkv[:, :, :, :g].flatten(2, 3), qkv[:, :, :, g], qkv[:, :, :, g + 1]
     k_cache.index_copy_(1, write_idx, k)
     v_cache.index_copy_(1, write_idx, v)
     return attention_decode(q, k_cache, v_cache, additive_mask, scale)
 
 
 def attention_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, additive_mask: torch.Tensor, scale: float) -> torch.Tensor:
-    """q [B,1,H,D] against the whole static cache [B,Lmax,H,D]; ``additive_mask`` ([B,1,1,Lmax] or [B,Lmax]) hides padded and
-    not-yet-written positions.  CPU / fallback: the plain softmax expression (also the numerical reference in the tests)."""
+    """q [B,1,H,D] against the whole static cache [B,Lmax,Hkv,D] (query head h reads cache head h // (H // Hkv)); ``additive_mask``
+    ([B,1,1,Lmax] or [B,Lmax]) hides padded and not-yet-written positions.  CPU / fallback: the plain softmax expression (also the
+    numerical reference in the tests)."""
     if q.is_cuda and _native.available():
         _count()
         return _native.require().attention_decode(q.contiguous(), k_cache, v_cache, additive_mask, k_cache.shape[1], float(scale))
+    if k_cache.shape[2] != q.shape[2]:
+        g = q.shape[2] // k_cache.shape[2]
+        k_cache, v_cache = k_cache.repeat_interleave(g, dim=2), v_cache.repeat_interleave(g, dim=2)
     s = torch.einsum("bqhd,bkhd->bhqk", q.float(), k_cache.float()) * scale + additive_mask.reshape(q.shape[0], 1, 1, -1).float()
     return torch.einsum("bhqk,bkhd->bqhd", torch.softmax(s, -1), v_cache.float()).to(q.dtype)
 

@@ -17,6 +17,25 @@ def check_device(device: str):
         raise ValueError(f"unsupported device '{device}': this framework targets NVIDIA H100 (gpu) with a cpu functional path")
 
 
+def check_kv_heads(m, d, compress) -> None:
+    """``Model.num_key_value_heads`` (grouped-query attention; unset = ``num_attention_heads``)."""
+    heads, kv = m.get("num_attention_heads"), m.get("num_key_value_heads")
+    if kv is None or not heads:
+        return
+    if kv < 1 or heads % kv:
+        raise ValueError(f"num_attention_heads ({heads}) must be a multiple of num_key_value_heads ({kv})")
+    if d.get("mp_degree", 1) > 1 and kv % d.mp_degree:
+        raise ValueError(f"num_key_value_heads ({kv}) must be divisible by mp_degree ({d.mp_degree}): tensor parallelism shards whole K/V groups")
+    if kv == heads:
+        return
+    if d.get("cp_degree", 1) > 1:
+        raise ValueError("num_key_value_heads < num_attention_heads is not supported with context parallelism (Distributed.cp_degree > 1)")
+    prune = compress.get("Prune") or {}
+    if prune.get("enable", False) and prune.get("prune_heads", True):
+        raise ValueError("Compress.Prune head pruning does not support num_key_value_heads < num_attention_heads; "
+                         "set Compress.Prune.prune_heads=False to prune the FFN only")
+
+
 def check_config(cfg):
     g, d = cfg.Global, cfg.get("Distributed", {})
     for key in ("local_batch_size", "micro_batch_size"):
@@ -34,5 +53,6 @@ def check_config(cfg):
         raise ValueError("hidden_size must be divisible by num_attention_heads")
     if m.get("num_attention_heads") and d.get("mp_degree", 1) > 1 and m.num_attention_heads % d.mp_degree:
         raise ValueError("num_attention_heads must be divisible by mp_degree")
+    check_kv_heads(m, d, cfg.get("Compress", {}) or {})
     logger.debug("config checks passed")
     return True

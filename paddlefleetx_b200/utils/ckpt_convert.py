@@ -185,7 +185,9 @@ def gpt_plain_to_pipe(state: dict, num_layers: int) -> dict:
     return out
 
 
-def convert(src: str, dst: str, mp: int = 1, to_plain_layers: Optional[int] = None, fuse_qkv: Optional[bool] = None, num_heads: Optional[int] = None):
+def convert(src: str, dst: str, mp: int = 1, to_plain_layers: Optional[int] = None, fuse_qkv: Optional[bool] = None, num_heads: Optional[int] = None,
+            num_kv_heads: Optional[int] = None):
+    """``num_kv_heads``: K/V heads of a grouped-query model (default ``num_heads``), used by the QKV re-layout."""
     model, optim, meta = merge_checkpoint(src)
     if to_plain_layers is not None:
         model = gpt_pipe_to_plain(model, to_plain_layers)
@@ -196,6 +198,6 @@ def convert(src: str, dst: str, mp: int = 1, to_plain_layers: Optional[int] = No
         from ..models.language_model.finetune_module import convert_qkv_layout
 
         assert num_heads, "--num-heads is required with --fuse-qkv/--split-qkv"
-        model = convert_qkv_layout(model, fuse_qkv, num_heads)
+        model = convert_qkv_layout(model, fuse_qkv, num_heads, num_kv_heads)
         optim = None        # moments do not survive a re-layout of fused rows; restart the optimizer
     return split_checkpoint(model, optim, meta, dst, mp)

@@ -189,6 +189,9 @@ def prune_model(model: nn.Module, cfg: dict) -> nn.Module:
             n_layers += 1
         attn = getattr(mod, "self_attn", None)
         if attn is not None and hasattr(attn, "qkv_proj") and cfg.get("prune_heads", True):
+            if getattr(attn, "group", 1) > 1:
+                raise ValueError("head pruning does not support grouped-query attention (num_key_value_heads < num_attention_heads); "
+                                 "set Compress.Prune.prune_heads=False to prune the FFN only")
             h, d = attn.local_heads, attn.head_dim
             keep_h = max(int(round(h * (1 - ratio))), 1)
             w = attn.qkv_proj.weight.data.view(h, 3 * d, -1)
@@ -199,6 +202,7 @@ def prune_model(model: nn.Module, cfg: dict) -> nn.Module:
             wo = attn.out_proj.weight.data.view(attn.out_proj.weight.shape[0], h, d)
             attn.out_proj.weight = nn.Parameter(wo[:, idx].reshape(wo.shape[0], keep_h * d).clone())
             attn.local_heads, attn.num_heads = keep_h, keep_h * getattr(attn, "world", 1)
+            attn.local_kv_heads, attn.num_kv_heads = attn.local_heads, attn.num_heads
     logger.info(f"pruned {n_layers} decoder layers with ratio {ratio} ({crit})")
     return model
 

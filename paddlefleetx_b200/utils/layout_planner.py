@@ -67,10 +67,21 @@ class ModelShape:
     ffn: int
     seq: int
     moe_experts: int = 0                 # experts per MoE layer on one rank (0 = dense)
+    kv_heads: int = 0                    # K/V heads (grouped-query attention); 0 = heads
+
+    @property
+    def n_kv_heads(self) -> int:
+        return self.kv_heads or self.heads
+
+    @property
+    def qkv_width(self) -> float:
+        """Output width of the fused QKV projection: (H + 2 Hkv) d."""
+        return (self.heads + 2 * self.n_kv_heads) * (self.hidden / self.heads)
 
     @property
     def params_per_layer(self) -> float:
-        return 4 * self.hidden * self.hidden + 2 * self.hidden * self.ffn + 9 * self.hidden + self.ffn
+        # QKV h (H + 2 Hkv) d, out-proj h^2, FFN 2 h f; biases (H + 2 Hkv) d + h + h + f, two norms 4 h
+        return self.hidden * self.qkv_width + self.hidden * self.hidden + 2 * self.hidden * self.ffn + self.qkv_width + 6 * self.hidden + self.ffn
 
     @property
     def params(self) -> float:
@@ -86,7 +97,8 @@ class ModelShape:
         except (AttributeError, KeyError):
             pass
         return ModelShape(layers=int(m.get("num_layers", m.get("num_hidden_layers", 12))), hidden=h, heads=int(m.get("num_attention_heads", 12)),
-                          vocab=int(m.get("vocab_size", 50304)), ffn=int(m.get("ffn_hidden_size", 4 * h) or 4 * h), seq=seq)
+                          vocab=int(m.get("vocab_size", 50304)), ffn=int(m.get("ffn_hidden_size", 4 * h) or 4 * h), seq=seq,
+                          kv_heads=int(m.get("num_key_value_heads") or 0))
 
 
 @dataclass
@@ -135,7 +147,7 @@ def _gemm_time(hw: Hardware, m: float, n: float, k: float) -> float:
 def _layer_time(hw: Hardware, s: ModelShape, tokens: float, mp: int, sp: bool, recompute: str) -> Dict[str, float]:
     """Forward + backward of one transformer layer for ``tokens`` tokens on one GPU of an ``mp``-way tensor-parallel group."""
     h, f = s.hidden, s.ffn
-    fwd_gemm = (_gemm_time(hw, tokens, 3 * h / mp, h) + _gemm_time(hw, tokens, h, h / mp)
+    fwd_gemm = (_gemm_time(hw, tokens, s.qkv_width / mp, h) + _gemm_time(hw, tokens, h, h / mp)
                 + _gemm_time(hw, tokens, f / mp, h) + _gemm_time(hw, tokens, h, f / mp))
     gemm = 3.0 * fwd_gemm                                        # dgrad + wgrad have the forward's shapes
     attn_flops = 2.0 * 2.0 * tokens * s.seq * h / mp / 2.0       # causal: half of QK^T and PV
@@ -144,7 +156,7 @@ def _layer_time(hw: Hardware, s: ModelShape, tokens: float, mp: int, sp: bool, r
     # column sums, residual adds: ~0.6 ms per layer at 8192 tokens) is ~120 h bytes per token
     tok_local = tokens / (mp if sp else 1)
     elem = 120.0 * h * tok_local / hw.hbm_bw
-    extra = {"none": 0.0, "core_attn": attn_fwd, "full_attn": attn_fwd + _gemm_time(hw, tokens, 3 * h / mp, h) + _gemm_time(hw, tokens, h, h / mp),
+    extra = {"none": 0.0, "core_attn": attn_fwd, "full_attn": attn_fwd + _gemm_time(hw, tokens, s.qkv_width / mp, h) + _gemm_time(hw, tokens, h, h / mp),
              "full": fwd_gemm + attn_fwd + elem / 3.0}[recompute]
     return {"gemm": gemm, "attn": attn_fwd + attn_bwd, "elementwise": elem, "recompute": extra}
 
@@ -224,7 +236,7 @@ def enumerate_plans(s: ModelShape, world: int, local_batch: int, stages: Iterabl
     ``local_batch`` is the per-GPU batch: a data rank of an (mp, pp) layout carries ``local_batch * mp * pp`` sequences."""
     out = []
     for mp in _divisors(world):
-        if s.heads % mp or s.hidden % mp or s.vocab % mp or mp > 8:
+        if s.heads % mp or s.n_kv_heads % mp or s.hidden % mp or s.vocab % mp or mp > 8:
             continue
         for pp in _divisors(world // mp):
             if s.layers % pp or (pp > 1 and not allow_pp):
@@ -238,7 +250,7 @@ def enumerate_plans(s: ModelShape, world: int, local_batch: int, stages: Iterabl
                         continue                                           # the stage-3 wrapper and the pipeline schedule are not combined
                     cps = [(1, "ulysses")]                                 # context parallelism only where long sequences make activations the problem
                     for c in _divisors(rest):
-                        if c > 1 and pp == 1 and s.seq >= 4096:           # (cp also runs under the pipeline schedule; not searched: RoPE models cannot use it)
+                        if c > 1 and pp == 1 and s.seq >= 4096 and s.n_kv_heads == s.heads:   # (cp also runs under the pipeline schedule; not searched: RoPE models cannot use it; nor can grouped K/V heads)
                             if (s.heads // mp) % c == 0 and s.seq % c == 0:
                                 cps.append((c, "ulysses"))
                             if s.seq % (2 * c) == 0:                       # zigzag shards: two chunks per rank

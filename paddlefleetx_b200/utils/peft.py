@@ -118,7 +118,7 @@ def apply_prefix_tuning(gpt_model: nn.Module, num_virtual_tokens: int = 16, hidd
     layers = gpt_model.decoder.layers
     att0 = layers[0].self_attn
     w = gpt_model.decoder.norm.weight
-    enc = PrefixEncoder(len(layers), att0.local_heads, att0.head_dim, num_virtual_tokens, hidden, reparam, w.dtype, w.device)
+    enc = PrefixEncoder(len(layers), getattr(att0, "local_kv_heads", att0.local_heads), att0.head_dim, num_virtual_tokens, hidden, reparam, w.dtype, w.device)
     gpt_model.prefix_encoder = enc
     for i, layer in enumerate(layers):
         _patch_attention(layer.self_attn, enc, i)
@@ -129,7 +129,7 @@ def _patch_attention(attn, enc: PrefixEncoder, index: int) -> None:
     import torch.nn.functional as F
 
     def core(q, k, v, attn_mask):
-        pk, pv = enc()[index]                                  # [heads, tokens, d]
+        pk, pv = enc()[index]                                  # [kv heads, tokens, d]
         b = q.shape[0]
         pk = pk.transpose(0, 1).unsqueeze(0).expand(b, -1, -1, -1).to(q.dtype)     # [b, tokens, heads, d]
         pv = pv.transpose(0, 1).unsqueeze(0).expand(b, -1, -1, -1).to(q.dtype)
@@ -137,8 +137,9 @@ def _patch_attention(attn, enc: PrefixEncoder, index: int) -> None:
         sq, sk, t = q.shape[1], k.shape[1], pk.shape[1]
         causal = torch.ones(sq, sk, dtype=torch.bool, device=q.device).tril(sk - sq)
         mask = torch.cat([torch.ones(sq, t, dtype=torch.bool, device=q.device), causal], 1)
+        gqa = {"enable_gqa": True} if k2.shape[2] != q.shape[2] else {}
         o = F.scaled_dot_product_attention(q.transpose(1, 2), k2.transpose(1, 2), v2.transpose(1, 2), attn_mask=mask,
-                                           dropout_p=attn.attn_dropout if attn.training else 0.0)
+                                           dropout_p=attn.attn_dropout if attn.training else 0.0, **gqa)
         return o.transpose(1, 2)
 
     attn._core = core

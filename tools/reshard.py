@@ -23,11 +23,12 @@ def main():
     g.add_argument("--fuse-qkv", action="store_true")
     g.add_argument("--split-qkv", action="store_true")
     p.add_argument("--num-heads", type=int, default=None)
+    p.add_argument("--num-kv-heads", type=int, default=None, help="K/V heads of a grouped-query model (default: --num-heads)")
     a = p.parse_args()
     fuse = True if a.fuse_qkv else (False if a.split_qkv else None)
     if a.to_plain and a.num_layers is None:
         p.error("--to-plain needs --num-layers")
-    out = convert(a.src, a.dst, a.mp, a.num_layers if a.to_plain else None, fuse, a.num_heads)
+    out = convert(a.src, a.dst, a.mp, a.num_layers if a.to_plain else None, fuse, a.num_heads, a.num_kv_heads)
     print(f"wrote {out}")
 
 
