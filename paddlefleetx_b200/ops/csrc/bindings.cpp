@@ -22,6 +22,13 @@ inline int dtype_code(const at::Tensor& t) {
   }
 }
 inline bool is_16bit(const at::Tensor& t) { return t.scalar_type() == at::kBFloat16 || t.scalar_type() == at::kHalf; }
+// The bandwidth-bound kernels are compiled for bf16 and fp16 only; any other dtype would be reinterpreted as one of them.
+inline void check_16bit(const at::Tensor& t, const char* op, const char* name) {
+  TORCH_CHECK(is_16bit(t), op, ": ", name, " must be bf16 or fp16, got ", t.scalar_type());
+}
+inline void check_like(const at::Tensor& t, const at::Tensor& ref, const char* op, const char* name) {
+  TORCH_CHECK(t.scalar_type() == ref.scalar_type(), op, ": ", name, " dtype ", t.scalar_type(), " differs from ", ref.scalar_type());
+}
 inline cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
 inline int num_sms() {
   static int n = 0;
@@ -246,8 +253,17 @@ at::Tensor gemm_mxfp8(const at::Tensor& a, const at::Tensor& sfa, const at::Tens
 // ------------------------------------------------------------------------------- norms
 std::vector<at::Tensor> norm_fwd(const at::Tensor& x, const at::Tensor& w, c10::optional<at::Tensor> b, double eps, bool rms) {
   PFX_CHECK_CUDA_CONTIG(x); PFX_CHECK_CUDA_CONTIG(w);
-  const c10::cuda::CUDAGuard guard(x.device());
+  check_16bit(x, "norm_fwd", "x");
   const int64_t cols = x.size(-1), rows = x.numel() / cols;
+  TORCH_CHECK(cols % 8 == 0 && cols <= 32768, "norm_fwd: the row length must be a multiple of 8 and at most 32768, got ", cols);
+  check_like(w, x, "norm_fwd", "w");
+  TORCH_CHECK(w.numel() == cols, "norm_fwd: w has ", w.numel(), " elements for rows of ", cols);
+  if (b.has_value() && b->defined()) {
+    PFX_CHECK_CUDA_CONTIG(*b);
+    check_like(*b, x, "norm_fwd", "b");
+    TORCH_CHECK(b->numel() == cols, "norm_fwd: b has ", b->numel(), " elements for rows of ", cols);
+  }
+  const c10::cuda::CUDAGuard guard(x.device());
   auto y = at::empty_like(x);
   auto fopt = x.options().dtype(at::kFloat);
   auto mean = rms ? at::empty({0}, fopt) : at::empty({rows}, fopt);
@@ -261,7 +277,14 @@ std::vector<at::Tensor> norm_fwd(const at::Tensor& x, const at::Tensor& w, c10::
 std::vector<at::Tensor> norm_bwd(const at::Tensor& dy, const at::Tensor& x, const at::Tensor& w, const at::Tensor& mean,
                                  const at::Tensor& rstd, bool rms, bool has_bias, c10::optional<at::Tensor> dres) {
   // dres: gradient of the residual branch that bypasses the norm (pre-norm block): dx = norm_bwd(dy) + dres in the same pass
-  PFX_CHECK_CUDA_CONTIG(dy); PFX_CHECK_CUDA_CONTIG(x);
+  PFX_CHECK_CUDA_CONTIG(dy); PFX_CHECK_CUDA_CONTIG(x); PFX_CHECK_CUDA_CONTIG(w);
+  check_16bit(x, "norm_bwd", "x");
+  check_like(dy, x, "norm_bwd", "dy");
+  check_like(w, x, "norm_bwd", "w");
+  TORCH_CHECK(dy.sizes() == x.sizes(), "norm_bwd: dy shape ", dy.sizes(), " differs from x ", x.sizes());
+  TORCH_CHECK(x.size(-1) % 8 == 0 && x.size(-1) <= 32768, "norm_bwd: the row length must be a multiple of 8 and at most 32768, got ",
+              x.size(-1));
+  TORCH_CHECK(w.numel() == x.size(-1), "norm_bwd: w has ", w.numel(), " elements for rows of ", x.size(-1));
   const bool with_res = dres.has_value() && dres->defined();
   if (with_res) TORCH_CHECK(dres->is_contiguous() && dres->sizes() == x.sizes() && dres->scalar_type() == x.scalar_type(), "norm_bwd: dres");
   const c10::cuda::CUDAGuard guard(x.device());
@@ -284,6 +307,7 @@ static void check_same_dtype(const at::Tensor& x, const c10::optional<at::Tensor
 }
 at::Tensor bias_gelu_fwd(const at::Tensor& x, c10::optional<at::Tensor> bias, bool exact) {
   PFX_CHECK_CUDA_CONTIG(x);
+  check_16bit(x, "bias_gelu", "x");
   check_same_dtype(x, bias, "bias_gelu");
   const c10::cuda::CUDAGuard guard(x.device());
   auto y = at::empty_like(x);
@@ -294,6 +318,7 @@ at::Tensor bias_gelu_fwd(const at::Tensor& x, c10::optional<at::Tensor> bias, bo
 }
 at::Tensor bias_gelu_bwd(const at::Tensor& dy, const at::Tensor& x, c10::optional<at::Tensor> bias, bool exact) {
   PFX_CHECK_CUDA_CONTIG(x); PFX_CHECK_CUDA_CONTIG(dy);
+  check_16bit(x, "bias_gelu_bwd", "x");
   check_same_dtype(x, bias, "bias_gelu_bwd");
   TORCH_CHECK(dy.scalar_type() == x.scalar_type(), "bias_gelu_bwd: dy dtype");
   const c10::cuda::CUDAGuard guard(x.device());
@@ -306,6 +331,7 @@ at::Tensor bias_gelu_bwd(const at::Tensor& dy, const at::Tensor& x, c10::optiona
 at::Tensor bias_dropout_add_fwd(const at::Tensor& x, c10::optional<at::Tensor> bias, c10::optional<at::Tensor> residual, double p,
                                 int64_t seed, int64_t offset) {
   PFX_CHECK_CUDA_CONTIG(x);
+  check_16bit(x, "bias_dropout_add", "x");
   check_same_dtype(x, bias, "bias_dropout_add");
   check_same_dtype(x, residual, "bias_dropout_add");
   const c10::cuda::CUDAGuard guard(x.device());
@@ -320,6 +346,7 @@ at::Tensor bias_dropout_add_fwd(const at::Tensor& x, c10::optional<at::Tensor> b
 }
 at::Tensor dropout_bwd(const at::Tensor& dy, double p, int64_t seed, int64_t offset) {
   PFX_CHECK_CUDA_CONTIG(dy);
+  check_16bit(dy, "dropout_bwd", "dy");
   const c10::cuda::CUDAGuard guard(dy.device());
   auto dx = at::empty_like(dy);
   const int64_t cols = dy.size(-1);
@@ -329,6 +356,7 @@ at::Tensor dropout_bwd(const at::Tensor& dy, double p, int64_t seed, int64_t off
 }
 at::Tensor colsum(const at::Tensor& x, bool out_fp32) {
   PFX_CHECK_CUDA_CONTIG(x);
+  check_16bit(x, "colsum", "x");
   const c10::cuda::CUDAGuard guard(x.device());
   const int64_t cols = x.size(-1), rows = x.numel() / cols;
   auto out = at::empty({cols}, x.options().dtype(out_fp32 ? at::kFloat : x.scalar_type()));
@@ -340,9 +368,11 @@ at::Tensor colsum(const at::Tensor& x, bool out_fp32) {
 // ------------------------------------------------------------------------------- loss
 std::vector<at::Tensor> ce_stats(const at::Tensor& logits, const at::Tensor& labels, int64_t vocab_start) {
   PFX_CHECK_CUDA_CONTIG(logits); PFX_CHECK_CUDA_CONTIG(labels);
+  check_16bit(logits, "ce_stats", "logits");
   TORCH_CHECK(labels.scalar_type() == at::kLong, "labels must be int64");
   const c10::cuda::CUDAGuard guard(logits.device());
   const int64_t cols = logits.size(-1), rows = logits.numel() / cols;
+  TORCH_CHECK(labels.numel() == rows, "ce_stats: ", labels.numel(), " labels for ", rows, " rows");
   auto fopt = logits.options().dtype(at::kFloat);
   auto mx = at::empty({rows}, fopt), sm = at::empty({rows}, fopt), tg = at::empty({rows}, fopt);
   PFX_CUDA_CHECK(pfx::ce_stats(logits.data_ptr(), labels.data_ptr<int64_t>(), mx.data_ptr<float>(), sm.data_ptr<float>(),
@@ -350,9 +380,11 @@ std::vector<at::Tensor> ce_stats(const at::Tensor& logits, const at::Tensor& lab
   return {mx, sm, tg};
 }
 void ce_bwd_(at::Tensor& logits, const at::Tensor& labels, const at::Tensor& lse, const at::Tensor& gscale, int64_t vocab_start) {
-  PFX_CHECK_CUDA_CONTIG(logits);
+  PFX_CHECK_CUDA_CONTIG(logits); PFX_CHECK_CUDA_CONTIG(labels); PFX_CHECK_CUDA_CONTIG(lse); PFX_CHECK_CUDA_CONTIG(gscale);
+  check_16bit(logits, "ce_bwd_", "logits");
   const c10::cuda::CUDAGuard guard(logits.device());
   const int64_t cols = logits.size(-1), rows = logits.numel() / cols;
+  TORCH_CHECK(labels.scalar_type() == at::kLong && labels.numel() == rows, "ce_bwd_: labels must be int64 with one entry per row");
   TORCH_CHECK(lse.scalar_type() == at::kFloat && gscale.scalar_type() == at::kFloat && lse.numel() == rows && gscale.numel() == rows);
   PFX_CUDA_CHECK(pfx::ce_bwd(logits.data_ptr(), labels.data_ptr<int64_t>(), lse.data_ptr<float>(), gscale.data_ptr<float>(), (int)rows,
                              (int)cols, vocab_start, dtype_code(logits), cur_stream()));
@@ -376,12 +408,18 @@ void adamw_flat_(c10::optional<at::Tensor> p_lp, at::Tensor& master, const at::T
                  c10::optional<at::Tensor> found_inf, int64_t cta_budget) {
   // cta_budget > 0: grid size cap (the kernel is launched with cta_budget CTAs instead of 8 per SM) — used when the update runs on a side
   // stream underneath GEMMs and must not take the whole memory system
-  PFX_CHECK_CUDA_CONTIG(master); PFX_CHECK_CUDA_CONTIG(grad);
+  PFX_CHECK_CUDA_CONTIG(master); PFX_CHECK_CUDA_CONTIG(grad); PFX_CHECK_CUDA_CONTIG(m); PFX_CHECK_CUDA_CONTIG(v);
   const c10::cuda::CUDAGuard guard(master.device());
   const size_t n = master.numel();
   TORCH_CHECK((size_t)grad.numel() == n && (size_t)m.numel() == n && (size_t)v.numel() == n, "adamw: size mismatch");
   const float bc1 = 1.0 - std::pow(beta1, (double)step), bc2 = 1.0 - std::pow(beta2, (double)step);
   const bool has_lp = p_lp.has_value() && p_lp->defined();
+  if (has_lp) {
+    PFX_CHECK_CUDA_CONTIG(*p_lp);
+    TORCH_CHECK((size_t)p_lp->numel() == n, "adamw: p_lp has ", p_lp->numel(), " elements, master has ", n);
+    TORCH_CHECK(!is_16bit(grad) || !is_16bit(*p_lp) || p_lp->scalar_type() == grad.scalar_type(), "adamw: a ", grad.scalar_type(),
+                " grad needs p_lp of the same dtype or fp32, got ", p_lp->scalar_type());
+  }
   PFX_CUDA_CHECK(pfx::adamw_flat(has_lp ? p_lp->data_ptr() : nullptr, master.data_ptr<float>(), grad.data_ptr(), m.data_ptr<float>(),
                                  v.data_ptr<float>(), n, (float)lr, (float)beta1, (float)beta2, (float)eps, (float)wd, bc1, bc2,
                                  (gscale.has_value() && gscale->defined()) ? gscale->data_ptr<float>() : nullptr,
@@ -413,10 +451,15 @@ at::Tensor rope(const at::Tensor& x, c10::optional<at::Tensor> positions, int64_
   TORCH_CHECK(x.dim() >= 3, "rope: [..., heads, d]");
   const c10::cuda::CUDAGuard guard(x.device());
   const int64_t d = x.size(-1), heads = x.size(-2), tokens = x.numel() / (d * heads);
+  TORCH_CHECK(d % 2 == 0, "rope: head dim must be even, got ", d);
   auto y = at::empty_like(x);
   const int64_t* pos = nullptr;
   at::Tensor pc;
-  if (positions.has_value() && positions->defined()) { pc = positions->to(at::kLong).contiguous(); pos = pc.data_ptr<int64_t>(); }
+  if (positions.has_value() && positions->defined()) {
+    pc = positions->to(at::kLong).contiguous();
+    TORCH_CHECK(pc.numel() == tokens, "rope: ", pc.numel(), " positions for ", tokens, " tokens");
+    pos = pc.data_ptr<int64_t>();
+  }
   PFX_CUDA_CHECK(pfx::rope(x.data_ptr(), y.data_ptr(), pos, (size_t)tokens, (int)heads, (int)d, (int)seq_len, (float)base, bwd,
                            dtype_code(x), num_sms(), cur_stream()));
   return y;
@@ -432,6 +475,8 @@ at::Tensor causal_softmax_fwd(const at::Tensor& x, double scale) {
 }
 at::Tensor causal_softmax_bwd(const at::Tensor& dy, const at::Tensor& y, double scale) {
   PFX_CHECK_CUDA_CONTIG(dy); PFX_CHECK_CUDA_CONTIG(y);
+  check_like(dy, y, "causal_softmax_bwd", "dy");
+  TORCH_CHECK(dy.sizes() == y.sizes(), "causal_softmax_bwd: dy shape ", dy.sizes(), " differs from y ", y.sizes());
   const c10::cuda::CUDAGuard guard(y.device());
   const int64_t sk = y.size(-1), sq = y.size(-2), batch = y.numel() / (sk * sq);
   auto dx = at::empty_like(y);

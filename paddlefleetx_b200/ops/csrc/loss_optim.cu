@@ -11,13 +11,16 @@ namespace pfx {
 //   row_max = max_j x_j, row_sum = sum_j exp(x_j - row_max), tgt = x[label - vocab_start] (0 if the label
 // lives on another vocab shard).  The python side all-reduces (max / rescaled sum / tgt) over the
 // tensor-parallel group, exactly the three tiny exchanges of ParallelCrossEntropy.
-template <typename T>
+// kVec: rows are read as 16-byte vectors, which needs cols % 8 == 0 and a 16-byte aligned base (otherwise row 1 onwards is
+// misaligned); the scalar instantiation reads every element through the tail loop.
+// While a thread's running max is still -inf (masked logits) there is nothing to rescale: exp(-inf - -inf) would be NaN.
+template <typename T, bool kVec>
 __global__ void ce_stats_kernel(const T* __restrict__ logits, const int64_t* __restrict__ labels, float* __restrict__ row_max,
                                 float* __restrict__ row_sum, float* __restrict__ tgt, int cols, int64_t vocab_start) {
   __shared__ float scratch[33];
   const int row = blockIdx.x;
   const T* xr = logits + (size_t)row * cols;
-  const int nvec = cols >> 3;
+  const int nvec = kVec ? cols >> 3 : 0;
   float m = -INFINITY, s = 0.f;
   for (int vi = threadIdx.x; vi < nvec; vi += blockDim.x) {
     float v[8];
@@ -26,15 +29,17 @@ __global__ void ce_stats_kernel(const T* __restrict__ logits, const int64_t* __r
 #pragma unroll
     for (int j = 1; j < 8; ++j) lm = fmaxf(lm, v[j]);
     const float nm = fmaxf(m, lm);
+    if (nm == -INFINITY) continue;
     float acc = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc += __expf(v[j] - nm);
     s = s * __expf(m - nm) + acc;
     m = nm;
   }
-  for (int c = nvec * 8 + threadIdx.x; c < cols; c += blockDim.x) {  // tail (cols % 8)
+  for (int c = nvec * 8 + threadIdx.x; c < cols; c += blockDim.x) {  // tail (cols % 8), or the whole row when !kVec
     const float v = to_f32<T>(xr[c]);
     const float nm = fmaxf(m, v);
+    if (nm == -INFINITY) continue;
     s = s * __expf(m - nm) + __expf(v - nm);
     m = nm;
   }
@@ -50,12 +55,12 @@ __global__ void ce_stats_kernel(const T* __restrict__ logits, const int64_t* __r
 }
 
 // dlogits (in place) = (exp(x - lse) - onehot(label)) * gscale[row]
-template <typename T>
+template <typename T, bool kVec>
 __global__ void ce_bwd_kernel(T* __restrict__ logits, const int64_t* __restrict__ labels, const float* __restrict__ lse,
                               const float* __restrict__ gscale, int cols, int64_t vocab_start) {
   const int row = blockIdx.x;
   T* xr = logits + (size_t)row * cols;
-  const int nvec = cols >> 3;
+  const int nvec = kVec ? cols >> 3 : 0;
   const float l = lse[row], g = gscale[row];
   const int64_t lab = labels[row] - vocab_start;
   for (int vi = threadIdx.x; vi < nvec; vi += blockDim.x) {
@@ -76,18 +81,35 @@ __global__ void ce_bwd_kernel(T* __restrict__ logits, const int64_t* __restrict_
   }
 }
 
+static bool ce_vec_ok(const void* logits, int cols) { return cols % 8 == 0 && reinterpret_cast<uintptr_t>(logits) % 16 == 0; }
+
+template <typename T>
+static void ce_stats_t(const void* logits, const int64_t* labels, float* row_max, float* row_sum, float* tgt, int rows, int cols,
+                       int64_t vocab_start, cudaStream_t st) {
+  if (ce_vec_ok(logits, cols)) ce_stats_kernel<T, true><<<rows, 512, 0, st>>>((const T*)logits, labels, row_max, row_sum, tgt, cols, vocab_start);
+  else ce_stats_kernel<T, false><<<rows, 512, 0, st>>>((const T*)logits, labels, row_max, row_sum, tgt, cols, vocab_start);
+}
+template <typename T>
+static void ce_bwd_t(void* logits, const int64_t* labels, const float* lse, const float* gscale, int rows, int cols, int64_t vocab_start,
+                     cudaStream_t st) {
+  if (ce_vec_ok(logits, cols)) ce_bwd_kernel<T, true><<<rows, 512, 0, st>>>((T*)logits, labels, lse, gscale, cols, vocab_start);
+  else ce_bwd_kernel<T, false><<<rows, 512, 0, st>>>((T*)logits, labels, lse, gscale, cols, vocab_start);
+}
+
 cudaError_t ce_stats(const void* logits, const int64_t* labels, float* row_max, float* row_sum, float* tgt, int rows, int cols,
                      int64_t vocab_start, int dtype, cudaStream_t st) {
   if (!rows) return cudaSuccess;
-  if (dtype == 1) ce_stats_kernel<__nv_bfloat16><<<rows, 512, 0, st>>>((const __nv_bfloat16*)logits, labels, row_max, row_sum, tgt, cols, vocab_start);
-  else ce_stats_kernel<__half><<<rows, 512, 0, st>>>((const __half*)logits, labels, row_max, row_sum, tgt, cols, vocab_start);
+  if (dtype == 1) ce_stats_t<__nv_bfloat16>(logits, labels, row_max, row_sum, tgt, rows, cols, vocab_start, st);
+  else if (dtype == 0) ce_stats_t<__half>(logits, labels, row_max, row_sum, tgt, rows, cols, vocab_start, st);
+  else return cudaErrorInvalidValue;
   return cudaGetLastError();
 }
 cudaError_t ce_bwd(void* logits, const int64_t* labels, const float* lse, const float* gscale, int rows, int cols, int64_t vocab_start,
                    int dtype, cudaStream_t st) {
   if (!rows) return cudaSuccess;
-  if (dtype == 1) ce_bwd_kernel<__nv_bfloat16><<<rows, 512, 0, st>>>((__nv_bfloat16*)logits, labels, lse, gscale, cols, vocab_start);
-  else ce_bwd_kernel<__half><<<rows, 512, 0, st>>>((__half*)logits, labels, lse, gscale, cols, vocab_start);
+  if (dtype == 1) ce_bwd_t<__nv_bfloat16>(logits, labels, lse, gscale, rows, cols, vocab_start, st);
+  else if (dtype == 0) ce_bwd_t<__half>(logits, labels, lse, gscale, rows, cols, vocab_start, st);
+  else return cudaErrorInvalidValue;
   return cudaGetLastError();
 }
 
@@ -231,6 +253,8 @@ cudaError_t adamw_flat(void* p_lp, float* master, const void* grad, float* m, fl
   if ((reinterpret_cast<uintptr_t>(master) | reinterpret_cast<uintptr_t>(m) | reinterpret_cast<uintptr_t>(v)) & 15) return cudaErrorMisalignedAddress;
   if ((reinterpret_cast<uintptr_t>(grad) | reinterpret_cast<uintptr_t>(p_lp)) & 7) return cudaErrorMisalignedAddress;
 #define PFX_ADAM(TG, TP) adamw_kernel<TG, TP><<<grid, threads, 0, st>>>((TP*)p_lp, master, (const TG*)grad, m, v, n, lr, beta1, beta2, eps, wd, bc1, bc2, gscale, found_inf)
+  // a 16-bit gradient pairs with a low-precision copy of its own dtype or an fp32 one (3, also meaning "no copy")
+  if ((grad_dtype == 1 && lp_dtype == 0) || (grad_dtype == 0 && lp_dtype == 1)) return cudaErrorInvalidValue;
   if (grad_dtype == 3) { if (lp_dtype == 1) PFX_ADAM(float, __nv_bfloat16); else if (lp_dtype == 0) PFX_ADAM(float, __half); else PFX_ADAM(float, float); }
   else if (grad_dtype == 1) { if (lp_dtype == 1) PFX_ADAM(__nv_bfloat16, __nv_bfloat16); else PFX_ADAM(__nv_bfloat16, float); }
   else { if (lp_dtype == 0) PFX_ADAM(__half, __half); else PFX_ADAM(__half, float); }

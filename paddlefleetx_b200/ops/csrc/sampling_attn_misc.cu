@@ -175,11 +175,12 @@ __global__ void rope_kernel(const T* __restrict__ x, T* __restrict__ y, const in
     const int i = idx % half;
     const size_t th = idx / half;
     const size_t tok = th / heads;
-    const float pos = positions ? (float)positions[tok] : (float)(tok % seq_len);
-    const float inv_freq = __powf(base, -2.f * i / d);
-    float sn, cs;
-    __sincosf(pos * inv_freq, &sn, &cs);
-    sn *= sign;
+    // The angle and its sine / cosine in fp64: at positions in the tens of thousands the fast-math fp32 forms (__powf, __sincosf)
+    // are off by more than a 16-bit output can hide.  Double-precision functions are not replaced by --use_fast_math.
+    const double pos = positions ? (double)positions[tok] : (double)(tok % seq_len);
+    double sd, cd;
+    sincos(pos * pow((double)base, -2.0 * i / d), &sd, &cd);
+    const float sn = (float)sd * sign, cs = (float)cd;
     const T* xp = x + th * d;
     T* yp = y + th * d;
     const float a = to_f32<T>(xp[i]), b = to_f32<T>(xp[i + half]);
