@@ -188,32 +188,46 @@ at::Tensor gemm_ag(const at::Tensor& a_local, const at::Tensor& b, const at::Ten
 }
 
 // ------------------------------------------------------------------------------- 8-bit GEMMs
+// The quantiser keeps a row in registers: cols % 8 == 0 and cols <= 32768.
 std::vector<at::Tensor> quantize_rows(const at::Tensor& x, c10::optional<at::Tensor> smooth, bool fp8) {
   PFX_CHECK_CUDA_CONTIG(x);
+  check_16bit(x, "quantize_rows", "x");
   const c10::cuda::CUDAGuard guard(x.device());
-  const int64_t cols = x.size(-1), rows = x.numel() / cols;
+  const int64_t cols = x.size(-1), rows = cols ? x.numel() / cols : 0;
+  TORCH_CHECK(cols % 8 == 0 && cols > 0 && cols <= 32768, "quantize_rows: x needs 8 <= cols <= 32768 with cols % 8 == 0, got ", cols);
   auto q = at::empty(x.sizes(), x.options().dtype(fp8 ? at::kFloat8_e4m3fn : at::kChar));
   auto scale = at::empty({rows}, x.options().dtype(at::kFloat));
   const float* sm = nullptr;
   at::Tensor smc;
-  if (smooth.has_value() && smooth->defined()) { smc = smooth->to(at::kFloat).contiguous(); sm = smc.data_ptr<float>(); }
+  if (smooth.has_value() && smooth->defined()) {
+    TORCH_CHECK(smooth->device() == x.device() && smooth->numel() == cols, "quantize_rows: smooth must be [", cols, "] on ", x.device(), ", got ",
+                smooth->sizes(), " on ", smooth->device());
+    smc = smooth->to(at::kFloat).contiguous(); sm = smc.data_ptr<float>();
+  }
   PFX_CUDA_CHECK(pfx::quantize_rows(x.data_ptr(), sm, q.data_ptr(), scale.data_ptr<float>(), (int)rows, (int)cols, dtype_code(x), fp8, cur_stream()));
   return {q, scale};
 }
+// out_dtype: bf16 (default) or fp16; bias must have the output dtype.
 at::Tensor gemm_lowp(const at::Tensor& a, const at::Tensor& b, c10::optional<at::Tensor> row_scale, c10::optional<at::Tensor> col_scale,
-                     c10::optional<at::Tensor> bias, int64_t config) {
+                     c10::optional<at::Tensor> bias, int64_t config, c10::optional<at::ScalarType> out_dtype) {
   TORCH_CHECK(a.is_cuda() && b.is_cuda() && a.dim() == 2 && b.dim() == 2 && a.is_contiguous() && b.is_contiguous(), "gemm_lowp: contiguous 2-D CUDA operands");
   TORCH_CHECK(a.scalar_type() == b.scalar_type() && (a.scalar_type() == at::kChar || a.scalar_type() == at::kFloat8_e4m3fn), "gemm_lowp: int8 or fp8-e4m3 operands");
   const c10::cuda::CUDAGuard guard(a.device());
   const int64_t M = a.size(0), K = a.size(1), N = b.size(0);
   TORCH_CHECK(b.size(1) == K && K % 16 == 0 && N % 8 == 0, "gemm_lowp: K % 16 == 0 and N % 8 == 0 required");
-  auto d = at::empty({M, N}, a.options().dtype(at::kBFloat16));
+  const at::ScalarType od = out_dtype.value_or(at::kBFloat16);
+  TORCH_CHECK(od == at::kBFloat16 || od == at::kHalf, "gemm_lowp: out_dtype must be bf16 or fp16, got ", od);
+  auto d = at::empty({M, N}, a.options().dtype(od));
   pfx::LowpGemmArgs g{};
-  g.a = a.data_ptr(); g.b = b.data_ptr(); g.d = d.data_ptr();
+  g.a = a.data_ptr(); g.b = b.data_ptr(); g.d = d.data_ptr(); g.out_fp16 = od == at::kHalf;
   at::Tensor rs, cs;
   if (row_scale.has_value() && row_scale->defined()) { rs = row_scale->to(at::kFloat).contiguous(); TORCH_CHECK(rs.numel() == M); g.row_scale = rs.data_ptr<float>(); }
   if (col_scale.has_value() && col_scale->defined()) { cs = col_scale->to(at::kFloat).contiguous(); TORCH_CHECK(cs.numel() == N); g.col_scale = cs.data_ptr<float>(); }
-  if (bias.has_value() && bias->defined()) { TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->numel() == N); g.bias = bias->data_ptr(); }
+  if (bias.has_value() && bias->defined()) {
+    TORCH_CHECK(bias->is_cuda() && bias->is_contiguous() && bias->scalar_type() == od && bias->numel() == N, "gemm_lowp: bias must be a contiguous [",
+                N, "] CUDA tensor of the output dtype ", od, ", got ", bias->scalar_type(), " ", bias->sizes());
+    g.bias = bias->data_ptr();
+  }
   g.M = (int)M; g.N = (int)N; g.K = (int)K; g.lda = (int)K; g.ldb = (int)K; g.ldd = (int)N;
   g.kind = a.scalar_type() == at::kChar ? 1 : 2;
   g.num_sms = num_sms(); g.config = (int)config;
@@ -224,6 +238,7 @@ at::Tensor gemm_lowp(const at::Tensor& a, const at::Tensor& b, c10::optional<at:
 // MX block-scaled fp8: quantiser and GEMM.  quantize_mxfp8(x [R, K]) -> (q e4m3 [R, K], sf uint8 [ceil(R / 128), K / 128, 512])
 std::vector<at::Tensor> quantize_mxfp8(const at::Tensor& x) {
   TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.is_contiguous() && x.size(1) % 128 == 0, "quantize_mxfp8: contiguous [R, K], K % 128 == 0");
+  check_16bit(x, "quantize_mxfp8", "x");
   const c10::cuda::CUDAGuard guard(x.device());
   const int64_t R = x.size(0), K = x.size(1);
   at::Tensor q = at::empty({R, K}, x.options().dtype(at::kFloat8_e4m3fn));
@@ -231,7 +246,8 @@ std::vector<at::Tensor> quantize_mxfp8(const at::Tensor& x) {
   PFX_CUDA_CHECK(pfx::quantize_mxfp8(x.data_ptr(), q.data_ptr(), sf.data_ptr(), (int)R, (int)K, dtype_code(x), cur_stream()));
   return {q, sf};
 }
-// d [M, N] bf16 = (A_q * 2^(sfa - 127)) (B_q * 2^(sfb - 127))^T (+ bias), the scales applied per 32-element K block by the tensor core
+// d [M, N] bf16 = (A_q * 2^(sfa - 127)) (B_q * 2^(sfb - 127))^T (+ bias): each K = 32 partial product is scaled by its two block scales and
+// summed in fp32 registers (Hopper's tensor core has no block-scale mode)
 at::Tensor gemm_mxfp8(const at::Tensor& a, const at::Tensor& sfa, const at::Tensor& b, const at::Tensor& sfb, c10::optional<at::Tensor> bias) {
   TORCH_CHECK(a.is_cuda() && a.dim() == 2 && b.dim() == 2 && a.is_contiguous() && b.is_contiguous() && a.scalar_type() == at::kFloat8_e4m3fn &&
               b.scalar_type() == at::kFloat8_e4m3fn, "gemm_mxfp8: contiguous e4m3 operands");
@@ -651,14 +667,29 @@ at::Tensor gemv_fused(const at::Tensor& x, const at::Tensor& w, c10::optional<at
   return y;
 }
 
-at::Tensor gemv_w8a8(const at::Tensor& xq, const at::Tensor& wq, const at::Tensor& xs, const at::Tensor& ws, c10::optional<at::Tensor> bias) {
+at::Tensor gemv_w8a8(const at::Tensor& xq, const at::Tensor& wq, const at::Tensor& xs, const at::Tensor& ws, c10::optional<at::Tensor> bias,
+                     c10::optional<at::ScalarType> out_dtype) {
   TORCH_CHECK(xq.is_cuda() && xq.scalar_type() == at::kChar && wq.scalar_type() == at::kChar && xq.is_contiguous() && wq.is_contiguous() &&
               xq.dim() == 2 && wq.dim() == 2 && xq.size(1) == wq.size(1), "gemv_w8a8: int8 x [M,K], w [N,K]");
-  TORCH_CHECK(xs.scalar_type() == at::kFloat && ws.scalar_type() == at::kFloat && xs.numel() == xq.size(0) && ws.numel() == wq.size(0), "gemv_w8a8: scales");
-  at::Tensor y = at::empty({xq.size(0), wq.size(0)}, xq.options().dtype(at::kBFloat16));
-  const void* b = (bias.has_value() && bias->defined()) ? bias->data_ptr() : nullptr;
+  TORCH_CHECK(wq.is_cuda() && wq.device() == xq.device(), "gemv_w8a8: wq must be on ", xq.device());
+  // the kernel reads xq and wq rows with 16-byte loads
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(xq.data_ptr()) % 16 == 0, "gemv_w8a8: xq must be 16-byte aligned");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(wq.data_ptr()) % 16 == 0, "gemv_w8a8: wq must be 16-byte aligned");
+  TORCH_CHECK(xs.is_cuda() && xs.is_contiguous() && xs.scalar_type() == at::kFloat && xs.numel() == xq.size(0), "gemv_w8a8: xs must be a contiguous [",
+              xq.size(0), "] float CUDA tensor");
+  TORCH_CHECK(ws.is_cuda() && ws.is_contiguous() && ws.scalar_type() == at::kFloat && ws.numel() == wq.size(0), "gemv_w8a8: ws must be a contiguous [",
+              wq.size(0), "] float CUDA tensor");
+  const c10::cuda::CUDAGuard guard(xq.device());
+  const bool has_bias = bias.has_value() && bias->defined();
+  const at::ScalarType od = out_dtype.value_or(at::kBFloat16);
+  TORCH_CHECK(od == at::kBFloat16 || od == at::kHalf, "gemv_w8a8: out_dtype must be bf16 or fp16, got ", od);
+  if (has_bias)
+    TORCH_CHECK(bias->is_cuda() && bias->is_contiguous() && bias->scalar_type() == od && bias->numel() == wq.size(0), "gemv_w8a8: bias must be a contiguous [",
+                wq.size(0), "] CUDA tensor of the output dtype ", od, ", got ", bias->scalar_type(), " ", bias->sizes());
+  at::Tensor y = at::empty({xq.size(0), wq.size(0)}, xq.options().dtype(od));
+  const void* b = has_bias ? bias->data_ptr() : nullptr;
   PFX_CUDA_CHECK(pfx::gemv_w8a8(xq.data_ptr(), wq.data_ptr(), xs.data_ptr<float>(), ws.data_ptr<float>(), b, y.data_ptr(), (int)xq.size(0),
-                                (int)wq.size(0), (int)xq.size(1), at::cuda::getCurrentDeviceProperties()->multiProcessorCount, cur_stream()));
+                                (int)wq.size(0), (int)xq.size(1), num_sms(), cur_stream(), od == at::kHalf ? 0 : 1));
   return y;
 }
 
@@ -1021,7 +1052,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("gemm_ag", &gemm_ag);
   m.def("quantize_rows", &quantize_rows);
   m.def("gemm_lowp", &gemm_lowp, py::arg("a"), py::arg("b"), py::arg("row_scale") = py::none(), py::arg("col_scale") = py::none(),
-        py::arg("bias") = py::none(), py::arg("config") = 0);
+        py::arg("bias") = py::none(), py::arg("config") = 0, py::arg("out_dtype") = py::none());
   m.def("norm_fwd", &norm_fwd);
   m.def("norm_bwd", &norm_bwd, py::arg("dy"), py::arg("x"), py::arg("w"), py::arg("mean"), py::arg("rstd"), py::arg("rms"), py::arg("has_bias"),
         py::arg("dres") = py::none());
@@ -1072,7 +1103,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("gemm_dgelu", &gemm_dgelu);
   m.def("gemv_skinny", &gemv_skinny);
   m.def("gemm_smallm", &gemm_smallm);
-  m.def("gemv_w8a8", &gemv_w8a8);
+  m.def("gemv_w8a8", &gemv_w8a8, py::arg("xq"), py::arg("wq"), py::arg("xs"), py::arg("ws"), py::arg("bias") = py::none(),
+        py::arg("out_dtype") = py::none());
   m.def("gemv_fused", &gemv_fused);
   m.def("gemv_set_tuning", [](int64_t cols, int64_t split) { pfx::gemv_set_tuning((int)cols, (int)split); });
   m.def("moe_route", &moe_route);

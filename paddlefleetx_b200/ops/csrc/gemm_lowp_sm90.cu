@@ -1,13 +1,17 @@
 // 8-bit wgmma GEMMs for sm_90a: int8 x int8 -> int32 (the W8A8 inference GEMM behind the QAT / SmoothQuant export) and
 // fp8 e4m3 x e4m3 -> fp32 (the scaled TP GEMM).
 //
-//   D[M,N] (bf16) = (A_q[M,K] * B_q[N,K]^T) * row_scale[M] * col_scale[N] (+ bias[N])
+//   D[M,N] (bf16 or fp16) = (A_q[M,K] * B_q[N,K]^T) * row_scale[M] * col_scale[N] (+ bias[N], same dtype as D)
 //
 // Same pipeline as gemm_sm90.cu (TMA producer warp, two consumer warpgroups with the accumulator fragment in registers, swizzled smem
 // staging + TMA store, persistent grouped raster, 128 x 128 tiles) with the 8-bit specifics: 128 elements per 128-byte swizzle row
 // (BLOCK_K = 128), wgmma K = 32, integer accumulators are converted with I2F in the epilogue and the per-token / per-channel
 // dequantisation scales are applied there, so the int32 / fp32 product never touches HBM.  Reference: L23 in SURVEY §2.6
 // (Paddle-Inference / TensorRT int8 passes — no in-tree kernel in the reference).
+//
+// fp8 accumulation: the tensor core does not keep a full fp32 sum across an fp8 wgmma chain.  On an H100 a 128-K chain of positive
+// terms loses up to 2^-10 of their sum, and one chain over K = 16384 lost 25 % (tests/test_gpu_lowp_kernels.py).  Kind 2 therefore runs
+// one chain per k-block (128 K, one stage) into a fresh partial and adds it to the fp32 accumulator in registers.
 //
 // kKind 3 = MX block-scaled fp8: every 32 K-elements of every row of A and B carry their own E8M0 scale (2^(e - 127)).  Hopper's tensor
 // core has no block-scale mode, so each K = 32 wgmma writes a fresh partial product and the consumer threads fold it into the fp32
@@ -54,12 +58,13 @@ __device__ __forceinline__ void tile_of(int tile, int num_m, int num_n, int& m_b
 
 __device__ __forceinline__ float e8m0_to_float(uint32_t e) { return __uint_as_float(e == 0u ? 0x00400000u : e << 23); }
 
-// kKind: 1 = int8 (s32 accumulate), 2 = fp8 e4m3 (f32 accumulate), 3 = MX fp8 (per-32 block scales folded in by the consumers)
-template <int kKind>
+// kKind: 1 = int8 (s32 accumulate), 2 = fp8 e4m3 (f32 accumulate, promoted per k-block), 3 = MX fp8 (per-32 block scales folded in by
+// the consumers).  kBf16: D and bias are bf16, otherwise fp16.
+template <int kKind, bool kBf16>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_lowp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                  const __grid_constant__ CUtensorMap tmap_d, const float* __restrict__ row_scale, const float* __restrict__ col_scale,
-                 const __nv_bfloat16* __restrict__ bias, int M, int N, int K, const uint8_t* __restrict__ sfa, const uint8_t* __restrict__ sfb) {
+                 const void* __restrict__ bias, int M, int N, int K, const uint8_t* __restrict__ sfa, const uint8_t* __restrict__ sfb) {
   constexpr bool kMx = kKind == 3;
   using S = Smem<kMx>;
   using Acc = std::conditional_t<kKind == 1, int32_t, float>;
@@ -115,7 +120,7 @@ gemm_lowp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       int m_blk, n_blk; tile_of(tile, num_m, num_n, m_blk, n_blk);
       const int row0 = m_blk * kBlockM, col_tile = n_blk * kBlockN;
       Acc acc[kBlockN / 2];
-      if constexpr (kMx) {
+      if constexpr (kKind != 1) {
 #pragma unroll
         for (int i = 0; i < kBlockN / 2; ++i) acc[i] = 0;
       }
@@ -148,11 +153,23 @@ gemm_lowp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           }
           __syncwarp();
           if (lane == 0) mbar_arrive(empty_bar(stage));
+        } else if constexpr (kKind == 2) {
+          float part[kBlockN / 2];
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kBlockK / kMmaK; ++k)
+            Wgmma8<kBlockN, false>::mma(part, wgmma_desc(sa + k * kMmaK, kDesc), wgmma_desc(sb + k * kMmaK, kDesc), k != 0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<0>();
+#pragma unroll
+          for (int i = 0; i < kBlockN / 2; ++i) acc[i] += part[i];
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar(stage));
         } else {
           wgmma_fence();
 #pragma unroll
           for (int k = 0; k < kBlockK / kMmaK; ++k)        // 32 B per K = 32 step
-            Wgmma8<kBlockN, kKind == 1>::mma(acc, wgmma_desc(sa + k * kMmaK, kDesc), wgmma_desc(sb + k * kMmaK, kDesc), (kb | k) != 0 ? 1u : 0u);
+            Wgmma8<kBlockN, true>::mma(acc, wgmma_desc(sa + k * kMmaK, kDesc), wgmma_desc(sb + k * kMmaK, kDesc), (kb | k) != 0 ? 1u : 0u);
           wgmma_commit();
           if (prev_stage >= 0) {
             wgmma_wait<1>();
@@ -162,7 +179,7 @@ gemm_lowp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         }
         if (++stage == kStages) { stage = 0; phase ^= 1u; }
       }
-      if constexpr (!kMx) {
+      if constexpr (kKind == 1) {
         wgmma_wait<0>();
         if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar(prev_stage));
       }
@@ -184,7 +201,7 @@ gemm_lowp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
               v[4 * j] *= cs.x; v[4 * j + 1] *= cs.y; v[4 * j + 2] *= cs.x; v[4 * j + 3] *= cs.y;
             }
             if (bias) {
-              const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(bias + cb + 8 * j));
+              const float2 f = load_16x2<kBf16>(static_cast<const uint16_t*>(bias) + cb + 8 * j);
               v[4 * j] += f.x; v[4 * j + 1] += f.y; v[4 * j + 2] += f.x; v[4 * j + 3] += f.y;
             }
           }
@@ -200,7 +217,7 @@ gemm_lowp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           const uint32_t sbase = smem_epi + buf * S::kEpiBytes + r * 128u + col_in8 * 2u;
 #pragma unroll
           for (int j = 0; j < 8; ++j)
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sbase + (((uint32_t)j ^ (r & 7u)) << 4)), "r"(pack_bf16x2(v[4 * j + 2 * hh], v[4 * j + 2 * hh + 1])) : "memory");
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sbase + (((uint32_t)j ^ (r & 7u)) << 4)), "r"(pack_16x2<kBf16>(v[4 * j + 2 * hh], v[4 * j + 2 * hh + 1])) : "memory");
         }
         fence_proxy_async_smem();
         asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -215,16 +232,16 @@ gemm_lowp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   }
 }
 
-template <int kKind>
+template <int kKind, bool kBf16>
 static cudaError_t launch(const LowpGemmArgs& g, cudaStream_t stream) {
   using S = Smem<kKind == 3>;
   if (kKind == 3 && (g.sfa == nullptr || g.sfb == nullptr || g.K % kBlockK != 0)) return cudaErrorInvalidValue;
   CUtensorMap ta, tb, td;
   bool ok = make_tmap_2d(&ta, g.a, 1, 2, g.K, g.M, (uint64_t)g.lda, kBlockK, kBlockM);
   ok &= make_tmap_2d(&tb, g.b, 1, 2, g.K, g.N, (uint64_t)g.ldb, kBlockK, kBlockN);
-  ok &= make_tmap_2d(&td, g.d, 2, 1, g.N, g.M, (uint64_t)g.ldd * 2, kStoreCols, kBlockM);
+  ok &= make_tmap_2d(&td, g.d, 2, kBf16 ? 1 : 0, g.N, g.M, (uint64_t)g.ldd * 2, kStoreCols, kBlockM);
   if (!ok) return cudaErrorInvalidValue;
-  auto kern = gemm_lowp_kernel<kKind>;
+  auto kern = gemm_lowp_kernel<kKind, kBf16>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal);
@@ -235,7 +252,7 @@ static cudaError_t launch(const LowpGemmArgs& g, cudaStream_t stream) {
   int ctas = g.num_sms;
   if (ctas > tiles) ctas = tiles;
   if (ctas < 1) ctas = 1;
-  kern<<<ctas, kNumThreads, S::kTotal, stream>>>(ta, tb, td, g.row_scale, g.col_scale, reinterpret_cast<const __nv_bfloat16*>(g.bias), g.M, g.N, g.K,
+  kern<<<ctas, kNumThreads, S::kTotal, stream>>>(ta, tb, td, g.row_scale, g.col_scale, g.bias, g.M, g.N, g.K,
                                                  reinterpret_cast<const uint8_t*>(g.sfa), reinterpret_cast<const uint8_t*>(g.sfb));
   return cudaGetLastError();
 }
@@ -244,8 +261,10 @@ static cudaError_t launch(const LowpGemmArgs& g, cudaStream_t stream) {
 
 cudaError_t gemm_lowp_wgmma(const LowpGemmArgs& g, cudaStream_t stream) {
   if (g.M <= 0 || g.N <= 0 || g.K <= 0) return cudaSuccess;
-  if (g.kind == 3) return lowp::launch<3>(g, stream);
-  return g.kind == 1 ? lowp::launch<1>(g, stream) : lowp::launch<2>(g, stream);
+  if (g.kind == 3) return g.out_fp16 ? cudaErrorInvalidValue : lowp::launch<3, true>(g, stream);
+  if (g.kind == 1) return g.out_fp16 ? lowp::launch<1, false>(g, stream) : lowp::launch<1, true>(g, stream);
+  if (g.kind == 2) return g.out_fp16 ? lowp::launch<2, false>(g, stream) : lowp::launch<2, true>(g, stream);
+  return cudaErrorInvalidValue;
 }
 
 }  // namespace pfx

@@ -174,11 +174,12 @@ cudaError_t launch_rows(const T* x, const T* w, const T* bias, T* y, int N, int 
 
 // ---------------------------------------------------------------------------------------------------------------- W8A8 variant
 // int8 weights (per-output-channel scale) x int8 activations (per-row scale): half the weight bytes of the bf16 stream, dot
-// products on dp4a, dequantisation + bias in the finish.  Same warp layout as above (column groups x K-slices).
-template <int kRows, int kCols, int kSplit>
+// products on dp4a, dequantisation + bias in the finish.  Same warp layout as above (column groups x K-slices).  T (bf16 / fp16) is the
+// dtype of y and bias.
+template <typename T, int kRows, int kCols, int kSplit>
 __global__ void __launch_bounds__(256) gemv_w8a8_kernel(const int8_t* __restrict__ x, const int8_t* __restrict__ w, const float* __restrict__ xs,
-                                                        const float* __restrict__ ws, const __nv_bfloat16* __restrict__ bias,
-                                                        __nv_bfloat16* __restrict__ y, int N, int K) {
+                                                        const float* __restrict__ ws, const T* __restrict__ bias,
+                                                        T* __restrict__ y, int N, int K) {
   constexpr int kGroups = 8 / kSplit;
   __shared__ int red[8][kCols * kRows];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -250,14 +251,14 @@ __global__ void __launch_bounds__(256) gemv_w8a8_kernel(const int8_t* __restrict
     int v = 0;
 #pragma unroll
     for (int s2 = 0; s2 < kSplit; ++s2) v += red[g * kSplit + s2][cr];
-    const float f = (float)v * xs[r] * ws[n] + (bias ? __bfloat162float(bias[n]) : 0.f);
-    y[(size_t)r * N + n] = __float2bfloat16(f);
+    const float f = (float)v * xs[r] * ws[n] + (bias ? to_f32<T>(bias[n]) : 0.f);
+    y[(size_t)r * N + n] = from_f32<T>(f);
   }
 }
 
-template <int kRows>
-cudaError_t launch_w8a8_rows(const int8_t* x, const int8_t* w, const float* xs, const float* ws, const __nv_bfloat16* bias, __nv_bfloat16* y, int N,
-                             int K, int num_sms, cudaStream_t st) {
+template <typename T, int kRows>
+cudaError_t launch_w8a8_rows(const int8_t* x, const int8_t* w, const float* xs, const float* ws, const T* bias, T* y, int N, int K, int num_sms,
+                             cudaStream_t st) {
   const long target = (long)num_sms * 24;
   const long groups = (N + 1) / 2;
   int split = 1;
@@ -265,7 +266,7 @@ cudaError_t launch_w8a8_rows(const int8_t* x, const int8_t* w, const float* xs, 
 #define PFX_GW(S)                                                                                                             \
   do {                                                                                                                        \
     constexpr int kG = 8 / S;                                                                                                 \
-    gemv_w8a8_kernel<kRows, 2, S><<<(int)((groups + kG - 1) / kG), 256, 0, st>>>(x, w, xs, ws, bias, y, N, K);                  \
+    gemv_w8a8_kernel<T, kRows, 2, S><<<(int)((groups + kG - 1) / kG), 256, 0, st>>>(x, w, xs, ws, bias, y, N, K);                  \
     return cudaGetLastError();                                                                                                \
   } while (0)
   if (split == 1) PFX_GW(1);
@@ -307,22 +308,30 @@ cudaError_t gemv_skinny(const void* x, const void* w, const void* bias, void* y,
 
 void gemv_set_tuning(int cols, int split) { g_gemv_cols = cols; g_gemv_split = split; }
 
+namespace {
+template <typename T>
+cudaError_t launch_w8a8(const int8_t* x, const int8_t* w, const float* xs, const float* ws, const T* bb, T* yy, int M, int N, int K, int num_sms,
+                        cudaStream_t st) {
+  switch (M) {
+    case 1: return launch_w8a8_rows<T, 1>(x, w, xs, ws, bb, yy, N, K, num_sms, st);
+    case 2: return launch_w8a8_rows<T, 2>(x, w, xs, ws, bb, yy, N, K, num_sms, st);
+    case 3: return launch_w8a8_rows<T, 3>(x, w, xs, ws, bb, yy, N, K, num_sms, st);
+    case 4: return launch_w8a8_rows<T, 4>(x, w, xs, ws, bb, yy, N, K, num_sms, st);
+    case 5: return launch_w8a8_rows<T, 5>(x, w, xs, ws, bb, yy, N, K, num_sms, st);
+    case 6: return launch_w8a8_rows<T, 6>(x, w, xs, ws, bb, yy, N, K, num_sms, st);
+    case 7: return launch_w8a8_rows<T, 7>(x, w, xs, ws, bb, yy, N, K, num_sms, st);
+    default: return launch_w8a8_rows<T, 8>(x, w, xs, ws, bb, yy, N, K, num_sms, st);
+  }
+}
+}  // namespace
+
 cudaError_t gemv_w8a8(const void* x, const void* w, const float* xs, const float* ws, const void* bias, void* y, int M, int N, int K, int num_sms,
-                      cudaStream_t st) {
+                      cudaStream_t st, int dtype) {
   if (M < 1 || M > 8 || K % 16) return cudaErrorInvalidValue;
   const int8_t *xx = (const int8_t*)x, *ww = (const int8_t*)w;
-  const __nv_bfloat16* bb = (const __nv_bfloat16*)bias;
-  __nv_bfloat16* yy = (__nv_bfloat16*)y;
-  switch (M) {
-    case 1: return launch_w8a8_rows<1>(xx, ww, xs, ws, bb, yy, N, K, num_sms, st);
-    case 2: return launch_w8a8_rows<2>(xx, ww, xs, ws, bb, yy, N, K, num_sms, st);
-    case 3: return launch_w8a8_rows<3>(xx, ww, xs, ws, bb, yy, N, K, num_sms, st);
-    case 4: return launch_w8a8_rows<4>(xx, ww, xs, ws, bb, yy, N, K, num_sms, st);
-    case 5: return launch_w8a8_rows<5>(xx, ww, xs, ws, bb, yy, N, K, num_sms, st);
-    case 6: return launch_w8a8_rows<6>(xx, ww, xs, ws, bb, yy, N, K, num_sms, st);
-    case 7: return launch_w8a8_rows<7>(xx, ww, xs, ws, bb, yy, N, K, num_sms, st);
-    default: return launch_w8a8_rows<8>(xx, ww, xs, ws, bb, yy, N, K, num_sms, st);
-  }
+  if (dtype == 1) return launch_w8a8<__nv_bfloat16>(xx, ww, xs, ws, (const __nv_bfloat16*)bias, (__nv_bfloat16*)y, M, N, K, num_sms, st);
+  if (dtype == 0) return launch_w8a8<__half>(xx, ww, xs, ws, (const __half*)bias, (__half*)y, M, N, K, num_sms, st);
+  return cudaErrorInvalidValue;
 }
 
 }  // namespace pfx

@@ -64,17 +64,19 @@ struct GemmArgs {
 
 cudaError_t gemm_wgmma(const GemmArgs& args, cudaStream_t stream);
 
-// 8-bit GEMM: D(bf16)[M,N] = (A_q[M,K] * B_q[N,K]^T) * row_scale[M] * col_scale[N] (+ bias[N]); both operands K-major.
+// 8-bit GEMM: D[M,N] = (A_q[M,K] * B_q[N,K]^T) * row_scale[M] * col_scale[N] (+ bias[N]); both operands K-major.  D and bias are bf16,
+// or fp16 with out_fp16 (kinds 1 and 2).
 struct LowpGemmArgs {
   const void* a; const void* b; void* d;
   const float* row_scale;   // [M] or nullptr
   const float* col_scale;   // [N] or nullptr
-  const void* bias;         // [N] bf16 or nullptr
+  const void* bias;         // [N] of D's dtype, or nullptr
   int M, N, K, lda, ldb, ldd;
-  int kind;                 // 1 = int8 (kind::i8), 2 = fp8 e4m3 (kind::f8f6f4), 3 = MX block-scaled fp8 e4m3 (kind::mxf8f6f4.block_scale)
+  int kind;                 // 1 = int8 (s32 accumulate), 2 = fp8 e4m3 (f32), 3 = MX block-scaled fp8 e4m3 (scales folded in per K = 32)
   int num_sms, config;
   const void* sfa = nullptr;   // kind 3: E8M0 scale bytes of A / B, one 512-byte atom per (128 rows, 128 K): [row_blocks, K / 128, 512]
   const void* sfb = nullptr;
+  bool out_fp16 = false;
 };
 cudaError_t gemm_lowp_wgmma(const LowpGemmArgs& args, cudaStream_t stream);
 

@@ -59,8 +59,9 @@ cudaError_t gemv_skinny(const void* x, const void* w, const void* bias, void* y,
                         const void* ln_w = nullptr, const void* ln_b = nullptr, float ln_eps = 1e-5f, const void* residual = nullptr, int act = 0);
 
 void gemv_set_tuning(int cols, int split);
+// y and bias: dtype 1 = bf16, 0 = fp16
 cudaError_t gemv_w8a8(const void* x, const void* w, const float* xs, const float* ws, const void* bias, void* y, int M, int N, int K, int num_sms,
-                      cudaStream_t st);
+                      cudaStream_t st, int dtype = 1);
 
 // gemm_smallm_sm90.cu — swap-AB wgmma GEMM, split-K over a cluster with DSMEM reduction (1 <= M <= 128, bf16)
 cudaError_t gemm_smallm(const void* x, const void* w, const void* bias, void* y, int M, int N, int K, int dtype, int split, int num_sms,

@@ -109,7 +109,8 @@ __global__ void __launch_bounds__(256) quantize_mxfp8_kernel(const T* __restrict
 }  // namespace
 
 cudaError_t quantize_mxfp8(const void* x, void* q, void* sf, int rows, int K, int dtype, cudaStream_t st) {
-  if (K % 128 || rows < 1) return cudaErrorInvalidValue;
+  if (K % 128 || rows < 0) return cudaErrorInvalidValue;
+  if (rows == 0) return cudaSuccess;
   const int64_t n = (int64_t)rows * (K / 32);
   const unsigned grid = (unsigned)((n + 255) / 256);
   if (dtype == 1) quantize_mxfp8_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, (uint8_t*)q, (uint8_t*)sf, rows, K);

@@ -4,8 +4,9 @@
                   post-training SmoothQuant), activations quantised per token on the fly (``quantize_rows`` kernel, optional
                   SmoothQuant divisor), product dequantised in the GEMM epilogue.
 ``fp8_linear``  — fp8-e4m3 forward GEMM for tensor-parallel training layers; backward runs in bf16 (master path) — "fp8 on the TP GEMMs"
-                  of BASELINE config #3.  Two recipes: ``mx`` (OCP MX block scaling: one E8M0 scale per 32 K-elements, applied by the
-                  tensor core, ``kind::mxf8f6f4.block_scale``) and ``rowwise`` (per-token x per-channel fp32 scales in the epilogue).
+                  of BASELINE config #3.  Two recipes: ``mx`` (OCP MX block scaling: one E8M0 scale per 32 K-elements; Hopper's tensor
+                  core has no block-scale mode, so the GEMM folds each K = 32 partial product into fp32 with its two scales) and
+                  ``rowwise`` (per-token x per-channel fp32 scales in the epilogue).
 
 CPU / no-native fallbacks emulate the same arithmetic with torch ops so exported models are testable anywhere.
 """
@@ -35,20 +36,30 @@ def quantize_rows_reference(x: torch.Tensor, smooth: Optional[torch.Tensor], fp8
     if smooth is not None:
         xf = xf / smooth.float()
     qmax = 448.0 if fp8 else 127.0
-    scale = xf.abs().amax(-1).clamp(min=1e-12) / qmax
+    amax = xf.abs().amax(-1)
+    scale = torch.where(amax > 0, amax / qmax, torch.ones_like(amax))       # an all-zero row gets scale 1, as in the kernel
     scaled = xf / scale.unsqueeze(-1)
     if fp8:
-        return scaled.to(torch.float8_e4m3fn), scale
+        return scaled.clamp(-qmax, qmax).to(torch.float8_e4m3fn), scale
     return torch.clamp(torch.round(scaled), -127, 127).to(torch.int8), scale
 
 
+def _int8_matmul(xq: torch.Tensor, wq: torch.Tensor) -> torch.Tensor:
+    """Exact xq @ wq^T of int8 operands as float64: |sum| <= K * 2^14 is an integer far below 2^53 (fp32 is exact only to 2^24)."""
+    return xq.double() @ wq.double().t()
+
+
 class Int8Linear(nn.Module):
+    """``bias`` is kept in its own 16-bit dtype (the model's), so that an fp16 model's output is computed and rounded in fp16."""
+
     def __init__(self, weight_q: torch.Tensor, weight_scale: torch.Tensor, bias: Optional[torch.Tensor] = None,
                  smooth: Optional[torch.Tensor] = None, act_scale: Optional[float] = None):
         super().__init__()
         self.register_buffer("weight_q", weight_q.contiguous())
         self.register_buffer("weight_scale", weight_scale.float().contiguous())
-        self.register_buffer("bias", None if bias is None else bias.to(torch.bfloat16).contiguous())
+        if bias is not None and bias.dtype not in (torch.bfloat16, torch.float16):
+            bias = bias.to(torch.bfloat16)
+        self.register_buffer("bias", None if bias is None else bias.contiguous())
         self.register_buffer("smooth", None if smooth is None else smooth.float().contiguous())
         self.act_scale = act_scale               # static activation scale from QAT (None = dynamic per token)
         self.out_features, self.in_features = weight_q.shape
@@ -61,19 +72,22 @@ class Int8Linear(nn.Module):
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         shp = x.shape
         x2 = x.reshape(-1, shp[-1])
-        if x2.is_cuda and _native.use_native(x2) and x2.dtype in (torch.bfloat16, torch.float16) and shp[-1] % 16 == 0 and self.out_features % 8 == 0:
+        bias = self.bias if self.bias is None or self.bias.dtype == x.dtype else self.bias.to(x.dtype)
+        # quantize_rows keeps a row in registers: at most 32768 columns; wider layers take the torch path below
+        if x2.is_cuda and _native.use_native(x2) and x2.dtype in (torch.bfloat16, torch.float16) and shp[-1] % 16 == 0 \
+                and shp[-1] <= 32768 and self.out_features % 8 == 0:
             lib = _native.require()
             xq, xs = lib.quantize_rows(x2.contiguous(), self.smooth, False)
             if x2.shape[0] <= 8:          # decode: int8 weight stream on dp4a (csrc/gemv_skinny.cu)
-                y = lib.gemv_w8a8(xq, self.weight_q, xs, self.weight_scale, self.bias)
+                y = lib.gemv_w8a8(xq, self.weight_q, xs, self.weight_scale, bias, out_dtype=x2.dtype)
             else:
-                y = lib.gemm_lowp(xq, self.weight_q, xs, self.weight_scale, self.bias, 0)
+                y = lib.gemm_lowp(xq, self.weight_q, xs, self.weight_scale, bias, 0, out_dtype=x2.dtype)
             OF._count(2)
-            return y.view(*shp[:-1], self.out_features).to(x.dtype)
+            return y.view(*shp[:-1], self.out_features)
         xq, xs = quantize_rows_reference(x2, self.smooth)
-        y = (xq.float() @ self.weight_q.float().t()) * xs.unsqueeze(1) * self.weight_scale.unsqueeze(0)
-        if self.bias is not None:
-            y = y + self.bias.float()
+        y = _int8_matmul(xq, self.weight_q) * xs.double().unsqueeze(1) * self.weight_scale.double().unsqueeze(0)
+        if bias is not None:
+            y = y + bias.double()
         return y.to(x.dtype).view(*shp[:-1], self.out_features)
 
 
@@ -132,8 +146,8 @@ def quantize_mx_reference(x: torch.Tensor) -> torch.Tensor:
 
 
 class _MxFp8LinearFn(torch.autograd.Function):
-    """Forward GEMM on MX block-scaled fp8 operands (scales applied by the tensor core); backward in bf16 on the saved high-precision
-    operands, like the row-wise recipe."""
+    """Forward GEMM on MX block-scaled fp8 operands (each K = 32 partial product scaled and summed in fp32 by ``gemm_mxfp8``); backward
+    in bf16 on the saved high-precision operands, like the row-wise recipe."""
 
     @staticmethod
     def forward(ctx, x, weight, bias):
@@ -150,21 +164,23 @@ class _MxFp8LinearFn(torch.autograd.Function):
     backward = _Fp8LinearFn.backward
 
 
+def _straight_through(y: torch.Tensor, x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor]) -> torch.Tensor:
+    """Forward value y (bitwise), gradients as if the GEMM were the exact linear: exact - exact.detach() is exactly zero."""
+    exact = torch.nn.functional.linear(x, weight, bias)
+    return y.detach() + (exact - exact.detach())
+
+
 def fp8_linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None, recipe: str = "rowwise") -> torch.Tensor:
     native = x.is_cuda and x.dtype == torch.bfloat16 and _native.use_native(x)
+    b64 = 0.0 if bias is None else bias.double()
     if recipe == "mx" and weight.shape[1] % 128 == 0 and weight.shape[0] % 8 == 0:
         if native:
             return _MxFp8LinearFn.apply(x, weight, bias)
-        y = quantize_mx_reference(x.reshape(-1, x.shape[-1])) @ quantize_mx_reference(weight).t()
-        y = y.to(x.dtype).view(*x.shape[:-1], weight.shape[0])
-        exact = torch.nn.functional.linear(x, weight, bias)
-        return exact + (y + (0 if bias is None else bias) - exact).detach()
+        y = quantize_mx_reference(x.reshape(-1, x.shape[-1])).double() @ quantize_mx_reference(weight).double().t() + b64
+        return _straight_through(y.to(x.dtype).view(*x.shape[:-1], weight.shape[0]), x, weight, bias)
     if native and weight.shape[1] % 16 == 0 and weight.shape[0] % 8 == 0:
         return _Fp8LinearFn.apply(x, weight, bias)
     xq, xs = quantize_rows_reference(x.reshape(-1, x.shape[-1]), None, True)
     wq, ws = quantize_rows_reference(weight, None, True)
-    y = (xq.float() * xs.unsqueeze(1)) @ (wq.float() * ws.unsqueeze(1)).t()
-    y = y.to(x.dtype).view(*x.shape[:-1], weight.shape[0])
-    # straight-through: gradients flow as if the GEMM were exact
-    exact = torch.nn.functional.linear(x, weight, bias)
-    return exact + (y + (0 if bias is None else bias) - exact).detach()
+    y = (xq.double() @ wq.double().t()) * xs.double().unsqueeze(1) * ws.double().unsqueeze(0) + b64
+    return _straight_through(y.to(x.dtype).view(*x.shape[:-1], weight.shape[0]), x, weight, bias)

@@ -65,7 +65,7 @@ class ShiftSmoothInt8Linear(nn.Module):
             out_f, in_f = weight.shape
             self.register_buffer("shift", torch.zeros(in_f, dtype=weight.dtype, device=weight.device))
             self.inner = Int8Linear(torch.zeros(out_f, in_f, dtype=torch.int8, device=weight.device), torch.ones(out_f, device=weight.device),
-                                    torch.zeros(out_f, dtype=torch.bfloat16, device=weight.device), torch.ones(in_f, device=weight.device))
+                                    torch.zeros(out_f, dtype=weight.dtype, device=weight.device), torch.ones(in_f, device=weight.device))
             return
         w = weight.detach().float()
         z = ((stats.max + stats.min) / 2).to(w.device) if shift else torch.zeros(w.shape[1], device=w.device)
@@ -74,7 +74,7 @@ class ShiftSmoothInt8Linear(nn.Module):
         s = (amax.pow(alpha) / wmax.pow(1 - alpha)).clamp(min=1e-5)
         b = (bias.detach().float() if bias is not None else torch.zeros(w.shape[0], device=w.device)) + w @ z     # fold the shift
         self.register_buffer("shift", z.to(weight.dtype))
-        self.inner = Int8Linear.from_float(w, b.to(torch.bfloat16), smooth=s)
+        self.inner = Int8Linear.from_float(w, b.to(weight.dtype), smooth=s)
 
     @classmethod
     def empty(cls, out_features: int, in_features: int, dtype=torch.bfloat16, device=None) -> "ShiftSmoothInt8Linear":

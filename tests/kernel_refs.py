@@ -1,5 +1,6 @@
 """float64 references and error bounds for the bandwidth-bound kernels (norms, GELU, dropout, column sums, cross-entropy, AdamW,
-rotary embedding, causal softmax).  Nothing here needs CUDA: the references run on whatever device their inputs live on.
+rotary embedding, causal softmax) and for the 8-bit path (per-row and MX quantisers, int8 / fp8 / MX GEMMs, the W8A8 GEMV).  Nothing
+here needs CUDA: the references run on whatever device their inputs live on.
 
 Every reference takes the exact values a kernel was given (16-bit inputs upcast, never re-rounded) and computes in float64, so the only
 differences left are the kernel's own: fp32 arithmetic, approximate intrinsics and the final rounding to the output dtype.
@@ -229,3 +230,142 @@ def causal_softmax_bwd(dy, y, scale):
     keep = causal_mask(y.shape[-2], y.shape[-1], y.device)
     dy = dy * keep
     return scale * y * (dy - (dy * y).sum(-1, keepdim=True))
+
+
+# ---------------------------------------------------------------------------------------------------------------- 8-bit
+# The 8-bit references are exact or nearly so: an int8 x int8 sum over K is an integer below K * 2^14 << 2^53, products of e4m3 values
+# (and of MX block scales) are exact in float64, and the quantisers are deterministic functions of their input.
+E4M3_MAX = 448.0
+INT8_MAX = 127.0
+# quantize_rows computes scale = amax(x / smooth) / qmax with --use_fast_math division (x / smooth and amax / qmax, 2 ulp each) and
+# quantises with x * rcp(scale); the scale therefore lies within 4 fp32 ulp of the float64 value, and x / (smooth * scale) within 2^-20
+# relative of what the kernel rounds.
+QUANT_SCALE_ULPS = 4
+QUANT_REL = 2.0 ** -20
+# Epilogue of the 8-bit GEMMs and the W8A8 GEMV: I2F of the int32 sum, * row scale, * column scale, + bias, each an fp32 rounding.
+LOWP_EPILOGUE = 4 * FP32_U
+# In-chain error of one fp8 wgmma chain (128 K: four m64n128k32 instructions accumulating in the tensor core), relative to the sum of
+# |terms| in that chunk.  The PTX ISA does not document the accumulator's width.  Measured on an H100 80GB HBM3 (700 W), 2026-10-17:
+# 2^-10.1 at K = 128 for positive terms (test_gpu_lowp_kernels.py::test_fp8_gemm_accumulation).  A single chain over K = 16384 lost 2^-2.
+FP8_MMA = 2.0 ** -9
+
+
+def _e4m3_grid(a):
+    """quantum of e4m3fn around |a| (float64 array/tensor): 2^(floor(log2 a) - 3), subnormal quantum 2^-9 below 2^-6."""
+    ex = torch.floor(torch.log2(a.clamp(min=2.0 ** -6)))
+    return torch.exp2(ex - 3)
+
+
+def e4m3_rne(t):
+    """float64 values of the round-to-nearest-even, saturating (satfinite) e4m3fn conversion of the float64 tensor t."""
+    t = _d(t)
+    a = t.abs()
+    q = _e4m3_grid(a)
+    r = torch.round(a / q) * q            # torch.round rounds half to even
+    return torch.sign(t) * r.clamp(max=E4M3_MAX)
+
+
+def _near_e4m3_tie(t, rel=QUANT_REL):
+    a = _d(t).abs()
+    q = _e4m3_grid(a)
+    mid = (torch.floor(a / q) + 0.5) * q
+    return ((a - mid).abs() <= rel * a) & (a < E4M3_MAX + 16)
+
+
+def quantize_rows_check(x, smooth, q, scale, fp8):
+    """Check a per-row quantisation (``quantize_rows``) of x [rows, cols] element by element against float64.  Takes the kernel's own
+    ``scale`` for the element check, so ties and fast-math rounding of the scale cannot make it flaky.  Raises AssertionError."""
+    cols = x.shape[-1]
+    x64 = _d(x).reshape(-1, cols)
+    s64 = _d(smooth).reshape(1, cols) if smooth is not None else torch.ones((1, cols), dtype=torch.float64, device=x64.device)
+    sc = _d(scale).reshape(-1)
+    qv = _d(q.view(torch.float8_e4m3fn) if fp8 else q).reshape(-1, cols)
+    amax = (x64 / s64).abs().amax(-1) if cols else torch.zeros(x64.shape[0], dtype=torch.float64)
+    qmax = E4M3_MAX if fp8 else INT8_MAX
+    want = torch.where(amax > 0, amax / qmax, torch.ones_like(amax))
+    ulp = torch.exp2(torch.floor(torch.log2(want)) - 23)
+    bad = (sc - want).abs() > QUANT_SCALE_ULPS * ulp
+    if bad.any():
+        i = int(bad.nonzero()[0])
+        raise AssertionError(f"quantize_rows scale row {i}: got {sc[i].item()!r}, want {want[i].item()!r} (amax {amax[i].item()!r} / {qmax})")
+    zero = amax == 0
+    if (qv[zero] != 0).any():
+        raise AssertionError("quantize_rows: an all-zero row quantised to nonzero values")
+    t = x64 / (s64 * sc[:, None])
+    if fp8:
+        want_q = e4m3_rne(t)
+        bad = (qv != want_q) & ~_near_e4m3_tie(t)
+    else:
+        bad = ((qv - t).abs() > 0.5 + QUANT_REL * t.abs()) | (qv.abs() > INT8_MAX)
+    if bad.any():
+        r, c = (int(v) for v in bad.nonzero()[0])
+        raise AssertionError(f"quantize_rows q[{r}, {c}]: got {qv[r, c].item()!r} for x / (smooth * scale) = {t[r, c].item()!r}")
+
+
+def mx_sf_index(r, kb, K):
+    """Byte offset of the E8M0 scale of row r, 32-element K block kb in the [ceil(R / 128), K / 128, 512] atom layout."""
+    return ((r // 128) * (K // 128) + kb // 4) * 512 + (r % 32) * 16 + ((r % 128) // 32) * 4 + kb % 4
+
+
+def mx_encode_sf(e_biased, K):
+    """e_biased uint8 [R, K / 32] (row-major scale bytes) -> the atom layout, zeros for rows >= R."""
+    R = e_biased.shape[0]
+    out = torch.zeros(((R + 127) // 128) * (K // 128) * 512, dtype=torch.uint8)
+    r = torch.arange(R)[:, None].expand(R, K // 32)
+    kb = torch.arange(K // 32)[None, :].expand(R, K // 32)
+    out[mx_sf_index(r, kb, K).reshape(-1)] = e_biased.reshape(-1).cpu()
+    return out.view((R + 127) // 128, K // 128, 512)
+
+
+def mx_decode_sf(sf, R, K):
+    """Atom layout -> uint8 [R, K / 32] scale bytes."""
+    r = torch.arange(R)[:, None].expand(R, K // 32)
+    kb = torch.arange(K // 32)[None, :].expand(R, K // 32)
+    return sf.reshape(-1).cpu()[mx_sf_index(r, kb, K)]
+
+
+def mx_quantize_ref(x):
+    """OCP MX fp8 of x [R, K] (K % 128 == 0) -> (q e4m3fn [R, K], sf uint8 atoms) as ``quantize_mxfp8`` must produce them bit for bit:
+    per 32-element block the scale exponent e = ceil(log2(amax / 448)) clamped to [-127, 127] (-127 for a zero block), stored as e + 127,
+    and q = RNE-saturating e4m3 of x * 2^-e."""
+    R, K = x.shape
+    blocks = _d(x).cpu().reshape(R, K // 32, 32)
+    amax = blocks.abs().amax(-1)
+    e = torch.where(amax > 0, torch.ceil(torch.log2(amax / E4M3_MAX)), torch.full_like(amax, -127.0)).clamp(-127, 127)
+    q = e4m3_rne(blocks * torch.exp2(-e)[..., None]).reshape(R, K)
+    return q.to(torch.float8_e4m3fn), mx_encode_sf((e + 127).to(torch.uint8), K)
+
+
+def mx_dequant(q, sf):
+    """float64 values of MX operands: e4m3 values times 2^(byte - 127) per (row, 32-element block); byte 0 is 2^-127."""
+    R, K = q.shape
+    e = mx_decode_sf(sf, R, K).to(torch.float64) - 127
+    return (_d(q.view(torch.float8_e4m3fn)).cpu().reshape(R, K // 32, 32) * torch.exp2(e)[..., None]).reshape(R, K)
+
+
+def lowp_gemm_ref(a, b, row_scale=None, col_scale=None, bias=None):
+    """D = (a @ b^T) * row_scale[:, None] * col_scale[None, :] + bias in float64, for float64 operand values a [M, K], b [N, K] (int8
+    values, decoded e4m3 or MX-dequantised).  -> (ref, acc_scale, terms_scale): |acc| |rs| |cs| + |bias| bounds the epilogue's rounding,
+    sum|terms| |rs| |cs| + |bias| the in-chain error of a floating-point accumulation."""
+    a64, b64 = _d(a), _d(b)
+    acc = a64 @ b64.t()
+    terms = a64.abs() @ b64.abs().t()
+    mul = torch.ones((), dtype=torch.float64, device=acc.device)
+    if row_scale is not None:
+        mul = mul * _d(row_scale).reshape(-1, 1).to(acc.device)
+    if col_scale is not None:
+        mul = mul * _d(col_scale).reshape(1, -1).to(acc.device)
+    bb = _d(bias).reshape(1, -1).to(acc.device) if bias is not None else torch.zeros((), dtype=torch.float64, device=acc.device)
+    return acc * mul + bb, acc.abs() * mul.abs() + bb.abs(), terms * mul.abs() + bb.abs()
+
+
+def int8_gemm_bound(acc_scale):
+    """``assert_close`` arguments for the int8 GEMM and GEMV: the int32 sum is exact, so one rounding to the output (c = 1) plus the
+    epilogue's fp32 roundings."""
+    return dict(scale=acc_scale, approx=LOWP_EPILOGUE, c=1.0)
+
+
+def fp8_gemm_bound(terms_scale, K):
+    """``assert_close`` arguments for the fp8 and MX GEMMs: the usual c = 4 bound with an fp32 sum over K / 128 chunks and the in-chain
+    error ``FP8_MMA`` of each chunk, both relative to the sum of |terms|."""
+    return dict(scale=terms_scale, n=max(K // 128, 1), approx=FP8_MMA + LOWP_EPILOGUE)
