@@ -108,10 +108,9 @@ __device__ void ag_push_role(const GemmComm& c, int comm_cta, int num_comm_ctas,
   }
 }
 
-// kBf16 (== (ab_format == 1), fixed by the launcher): bias and aux (the saved pre-activation of EPI_DGELU) have the operands' 16-bit type and
-// are read as bf16 or fp16.  The wgmma form and the store packing still branch on the runtime ab_format, as they did before the fp16
-// instantiations existed: making them compile-time too moves ptxas's register allocation of the bf16 kernels (161 -> 162 registers in
-// out modes 0 and 3), and the bf16 code is kept exactly as it was measured.
+// kBf16 (fixed by the launcher from the operands' dtype): the wgmma form, the 16-bit output packing and the bias / aux (the saved
+// pre-activation of EPI_DGELU) loads are bf16, otherwise fp16.  The form must be a compile-time choice: a runtime branch between two
+// wgmma forms puts every wgmma of the k-block in its own branch arm, and ptxas then fences and waits on each one separately (C7519).
 // kOutMode: 0 = bf16/fp16 via TMA store, 1 = fp32 direct store, 2 = fp32 direct accumulate (D += acc),
 //           3 = bf16 scatter into the destination rank's staging buffer over NVLink (GEMM -> reduce-scatter)
 template <int kBlockN, bool kAK, bool kBK, int kOutMode, bool kBf16>
@@ -119,7 +118,7 @@ __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_a_local,
                   float* __restrict__ out_f32, const uint16_t* __restrict__ bias,
-                  int M, int N, int K, int ldd, int epilogue, uint32_t ab_format, const __grid_constant__ GemmComm comm,
+                  int M, int N, int K, int ldd, int epilogue, const __grid_constant__ GemmComm comm,
                   const __grid_constant__ PeerMaps peer_maps, const __grid_constant__ CUtensorMap tmap_d2,
                   const uint16_t* __restrict__ aux, int ld_aux, const __grid_constant__ GemmGroup grp) {
   using S = GemmSmem<kBlockN>;
@@ -262,8 +261,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         for (int k = 0; k < kBlockK / kMmaK; ++k) {
           const uint64_t da = wgmma_desc(sa + k * kAdvA, kDescA);
           const uint64_t db = wgmma_desc(sb + k * kAdvB, kDescB);
-          if (ab_format == 1) WgmmaSS<kBlockN, true, !kAK, !kBK>::mma(acc, da, db, (kb | k) != 0 ? 1u : 0u);
-          else WgmmaSS<kBlockN, false, !kAK, !kBK>::mma(acc, da, db, (kb | k) != 0 ? 1u : 0u);
+          WgmmaSS<kBlockN, kBf16, !kAK, !kBK>::mma(acc, da, db, (kb | k) != 0 ? 1u : 0u);
         }
         wgmma_commit();
         if (prev_stage >= 0) {   // one k-block stays in flight: the previous one has retired, hand its stage back to the producer
@@ -326,13 +324,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             const uint32_t sbase = smem_epi + buf * S::kEpiBytes + r * 128u + col_in8 * 2u;
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-              uint32_t p;
-              if (ab_format == 1) {
-                p = pack_bf16x2(v[4 * j + 2 * hh], v[4 * j + 2 * hh + 1]);
-              } else {
-                __half2 h2 = __floats2half2_rn(v[4 * j + 2 * hh], v[4 * j + 2 * hh + 1]);
-                p = *reinterpret_cast<uint32_t*>(&h2);
-              }
+              const uint32_t p = pack_16x2<kBf16>(v[4 * j + 2 * hh], v[4 * j + 2 * hh + 1]);
               asm volatile("st.shared.b32 [%0], %1;" ::"r"(sbase + (((uint32_t)j ^ (r & 7u)) << 4)), "r"(p) : "memory");
             }
           }
@@ -578,7 +570,7 @@ static cudaError_t launch_cfg(const GemmArgs& g, cudaStream_t stream) {
   cfg.dynamicSmemBytes = S::kTotal;
   cfg.stream = stream;
   const cudaError_t le = cudaLaunchKernelEx(&cfg, kern, ta, tb, td, tal, reinterpret_cast<float*>(g.d), reinterpret_cast<const uint16_t*>(g.bias),
-                            g.M, g.N, g.K, g.ldd, g.epilogue, (uint32_t)g.ab_format, g.comm, pm, td2,
+                            g.M, g.N, g.K, g.ldd, g.epilogue, g.comm, pm, td2,
                             reinterpret_cast<const uint16_t*>(g.aux), g.ld_aux, g.group);
   if (le != cudaSuccess) {
     fprintf(stderr, "pfx gemm: launch failed (%s): grid %d, smem %d B\n", cudaGetErrorString(le), ctas, S::kTotal);
@@ -607,7 +599,7 @@ static cudaError_t launch_out(const GemmArgs& g, cudaStream_t s) {
 
 cudaError_t gemm_wgmma(const GemmArgs& g, cudaStream_t stream) {
   if (g.M <= 0 || g.N <= 0 || g.K <= 0) return cudaSuccess;
-  return launch_out<128>(g, stream);   // 128 x 128 tiles: 64 accumulator registers per consumer thread (161-168 registers in all; four variants spill 32 bytes)
+  return launch_out<128>(g, stream);   // 128 x 128 tiles: 64 accumulator registers per consumer thread (162-168 registers in all; the eight out-mode-1 variants spill 44 bytes)
 }
 
 }  // namespace pfx

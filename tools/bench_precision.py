@@ -9,8 +9,11 @@ bracketed by synchronisation and CUDA events.  float16 trains with the dynamic l
 line reports the final scale and how many timed steps it skipped.  Every line carries the GPU name and power limit read in the same
 process (``nvidia-smi --query-gpu=name,power.limit``, read only).
 
-Kernel mode times the persistent GEMM at GPT-1.3B's Linear shapes (8 x 1024 tokens, hidden 2048: QKV, attention output, FFN1, FFN2 in the
-forward, dgrad and wgrad forms) and flash attention forward + backward at b 8, s 1024, h 16, d 128 (causal), in both dtypes.
+Kernel mode times the persistent GEMM at GPT-1.3B's Linear shapes (8 x 1024 tokens, hidden 2048: QKV, attention output, FFN1, FFN2 and
+the tied LM head with vocabulary 50304) in the forward and dgrad forms and in three wgrad forms: ``wgrad_bf16`` stores into a 16-bit
+[out, in] gradient buffer (out mode 0, what a training step without fp32 main gradients runs on a fresh gradient), ``wgrad_f32`` stores
+into an fp32 main gradient (out mode 1) and ``wgrad_f32acc`` accumulates into it (out mode 2).  Each row gives TFLOP/s and the share of
+the H100 SXM data-sheet dense rate (989 TFLOP/s).  Flash attention forward + backward runs at b 8, s 1024, h 16, d 128 (causal).  Both dtypes.
 """
 from __future__ import annotations
 
@@ -91,12 +94,18 @@ def run_arm(dtype: str, steps: int, warmup: int) -> dict:
                 loss_scale=scaler.get_scale() if scaler is not None else None, skipped_steps=skipped if scaler is not None else None, **gpu_info())
 
 
-def _time_ms(fn, iters=30, warmup=5) -> float:
+def _time_ms(fn, warmup=5, window_ms=500.0) -> float:
+    """Mean device time of one call over a window of at least ``window_ms`` (at least 30 calls): a few milliseconds of back-to-back
+    launches measure the clock state as much as the kernel."""
+    import time
+
     import torch
 
+    t0 = time.perf_counter()
     for _ in range(warmup):
         fn()
     torch.cuda.synchronize()
+    iters = max(30, int(window_ms / max((time.perf_counter() - t0) * 1e3 / warmup, 1e-3)))
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(iters):
@@ -113,7 +122,7 @@ def run_kernels() -> list:
 
     lib = _native.require()
     tokens, h = 8 * 1024, 2048
-    linears = {"qkv": (3 * h, h), "attn_out": (h, h), "ffn1": (4 * h, h), "ffn2": (h, 4 * h)}     # (out, in) features
+    linears = {"qkv": (3 * h, h), "attn_out": (h, h), "ffn1": (4 * h, h), "ffn2": (h, 4 * h), "lm_head": (50304, h)}   # (out, in) features
     rows = []
     info = gpu_info()
     for dt in (torch.float16, torch.bfloat16):
@@ -123,13 +132,18 @@ def run_kernels() -> list:
             w = torch.randn(n_out, n_in, device="cuda", dtype=dt) * 0.02
             dy = torch.randn(tokens, n_out, device="cuda", dtype=dt)
             main_grad = torch.zeros(n_out, n_in, device="cuda")
-            forms = {"fwd": lambda: lib.gemm(x, w, None, None, True, True, 0, 0, 0),                  # y = x W^T
-                     "dgrad": lambda: lib.gemm(dy, w, None, None, True, False, 0, 0, 0),              # dx = dy W
-                     "wgrad": lambda: lib.gemm(dy, x, None, main_grad, False, False, 0, 2, 0)}        # main_grad += dy^T x
+            grad = torch.empty(n_out, n_in, device="cuda", dtype=dt)
+            forms = {"fwd": lambda: lib.gemm(x, w, None, None, True, True, 0, 0, 0),                    # y = x W^T
+                     "dgrad": lambda: lib.gemm(dy, w, None, None, True, False, 0, 0, 0),                # dx = dy W
+                     "wgrad_bf16": lambda: lib.gemm(dy, x, None, grad, False, False, 0, 0, 0),          # grad = dy^T x (16-bit)
+                     "wgrad_f32": lambda: lib.gemm(dy, x, None, main_grad, False, False, 0, 1, 0),      # main_grad = dy^T x
+                     "wgrad_f32acc": lambda: lib.gemm(dy, x, None, main_grad, False, False, 0, 2, 0)}   # main_grad += dy^T x
             for form, fn in forms.items():
                 ms = _time_ms(fn)
-                rows.append(dict(kernel=f"gemm_{name}_{form}", dtype=str(dt).split(".")[-1], ms=round(ms, 4),
-                                 tflops=round(2.0 * tokens * n_out * n_in / ms / 1e9, 1), **info))
+                tflops = 2.0 * tokens * n_out * n_in / ms / 1e9
+                rows.append(dict(kernel=f"gemm_{name}_{form}", dtype=str(dt).split(".")[-1], ms=round(ms, 4), tflops=round(tflops, 1),
+                                 pct_of_989=round(100.0 * tflops / 989.0, 1), **info))
+            del x, w, dy, main_grad, grad
         b, s, nh, d = 8, 1024, 16, 128
         mix = torch.randn(b, s, nh, 3, d, device="cuda", dtype=dt)
         q, k, v = mix.unbind(3)
