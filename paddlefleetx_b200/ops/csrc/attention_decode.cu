@@ -3,7 +3,8 @@
 //   out[b, h, :] = softmax(scale * q[b, h, :] . K[b, 0:L, h, :] + mask[b, 0:L]) @ V[b, 0:L, h, :]
 //
 // q: [B, 1, H, D], K / V: [B, Lmax, H, D] (the framework's cache layout, read in place — no gather, no transpose), mask: additive
-// [B, Lmax] (0 = attend, large negative = padded / not yet written), D in {64, 128}.  One CTA per (head, batch): its warps take
+// [B, Lmax] (0 = attend, large negative or -inf = padded / not yet written), D in {64, 128}.  A row whose L keys are all masked with
+// -inf returns 0 (the flash kernels' l = 0 convention).  One CTA per (head, batch): its warps take
 // keys round-robin, every lane owns D/32 contiguous channels (one 4- or 8-byte load per key), the q.k dot product is a warp
 // shuffle reduction and each warp keeps a private online-softmax state (m, l, acc); the warps' partial states are merged through
 // shared memory at the end.  The op is a pure stream over the cache (2 * L * D * 2 bytes per head), so several keys are in flight
@@ -92,8 +93,9 @@ __global__ void __launch_bounds__(kDecWarps * 32) attention_decode_kernel(const 
       for (int o = kLanes / 2; o > 0; o >>= 1) sc += __shfl_xor_sync(0xffffffffu, sc, o);
       if (live) {
         if (mb) sc += to_f32<T>(mb[t]);
+        // a state whose keys so far are all masked with -inf has m = m_new = -inf: it must stay empty (l = 0), not turn into NaN
         const float m_new = fmaxf(m, sc);
-        const float corr = __expf(m - m_new), p = __expf(sc - m_new);
+        const float corr = (m == -INFINITY) ? 0.f : __expf(m - m_new), p = (sc == -INFINITY) ? 0.f : __expf(sc - m_new);
         l = l * corr + p;
 #pragma unroll
         for (int i = 0; i < 8; ++i) acc[i] = acc[i] * corr + p * vf[i];

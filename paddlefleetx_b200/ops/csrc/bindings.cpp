@@ -899,7 +899,8 @@ std::vector<at::Tensor> moe_dispatch(const at::Tensor& src, c10::optional<at::Te
                                    dtype_code(src), (int)num_ctas, cur_stream()));
   return {slot_loc, seg};
 }
-// Evoformer gated attention forward: q [G, Sq, H, 32], k / v [G, Sk, H, 32]; returns (out [G, Sq, H, 32], lse [G, H, Sq])
+// Evoformer gated attention forward: q [G, Sq, H, 32], k / v [G, Sk, H, 32]; returns (out [G, Sq, H, 32], stats [2, G, H, Sq]: row maximum and
+// log2 row sum, log2 units)
 std::vector<at::Tensor> evoformer_attention_fwd(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v, c10::optional<at::Tensor> mask_bias,
                                                 c10::optional<at::Tensor> pair_bias, c10::optional<at::Tensor> gate, int64_t groups_per_pair, double scale) {
   TORCH_CHECK(q.is_cuda() && q.dim() == 4 && k.dim() == 4 && v.dim() == 4 && q.is_contiguous() && k.is_contiguous() && v.is_contiguous(), "evoformer_attention: contiguous [G, S, H, 32]");
@@ -922,21 +923,22 @@ std::vector<at::Tensor> evoformer_attention_fwd(const at::Tensor& q, const at::T
     TORCH_CHECK(gate->scalar_type() == at::kBFloat16 && gate->is_contiguous() && gate->numel() == q.numel(), "evoformer_attention: gate bf16 like q");
     gt = gate->data_ptr();
   }
-  at::Tensor out = at::empty_like(q), lse = at::empty({G, H, Sq}, q.options().dtype(at::kFloat));
-  PFX_CUDA_CHECK(pfx::evoformer_attention_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr<float>(), mb, pb, gt, (int)G, (int)Sq,
+  at::Tensor out = at::empty_like(q), stats = at::empty({2, G, H, Sq}, q.options().dtype(at::kFloat));
+  PFX_CUDA_CHECK(pfx::evoformer_attention_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), stats.data_ptr<float>(), mb, pb, gt, (int)G, (int)Sq,
                                               (int)Sk, (int)H, (int)groups_per_pair, (float)scale, cur_stream()));
-  return {out, lse};
+  return {out, stats};
 }
 
 // Evoformer gated attention backward: returns (dq, dk, dv, dgate or empty, dpair fp32 or empty)
 std::vector<at::Tensor> evoformer_attention_bwd(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v, const at::Tensor& out, const at::Tensor& dout,
-                                                const at::Tensor& lse, c10::optional<at::Tensor> mask_bias, c10::optional<at::Tensor> pair_bias,
+                                                const at::Tensor& stats, c10::optional<at::Tensor> mask_bias, c10::optional<at::Tensor> pair_bias,
                                                 c10::optional<at::Tensor> gate, int64_t groups_per_pair, double scale, bool need_dpair) {
   TORCH_CHECK(q.is_cuda() && q.dim() == 4 && q.is_contiguous() && k.is_contiguous() && v.is_contiguous() && out.is_contiguous() && dout.is_contiguous() &&
               q.scalar_type() == at::kBFloat16 && dout.scalar_type() == at::kBFloat16 && out.sizes() == q.sizes() && dout.sizes() == q.sizes(),
               "evoformer_attention_bwd: contiguous bf16 [G, S, H, 32] operands");
   const int64_t G = q.size(0), Sq = q.size(1), H = q.size(2), Sk = k.size(1);
-  TORCH_CHECK(q.size(3) == 32 && H % 2 == 0 && lse.scalar_type() == at::kFloat && lse.numel() == G * H * Sq, "evoformer_attention_bwd: shapes");
+  TORCH_CHECK(q.size(3) == 32 && H % 2 == 0 && stats.scalar_type() == at::kFloat && stats.is_contiguous() && stats.numel() == 2 * G * H * Sq,
+              "evoformer_attention_bwd: shapes (stats: the forward's [2, G, H, Sq])");
   const c10::cuda::CUDAGuard guard(q.device());
   const bool has_gate = gate.has_value() && gate->defined(), has_pb = pair_bias.has_value() && pair_bias->defined(), has_mb = mask_bias.has_value() && mask_bias->defined();
   if (has_mb) TORCH_CHECK(mask_bias->scalar_type() == at::kFloat && mask_bias->is_contiguous() && mask_bias->numel() == G * Sk, "mask_bias fp32 [G, Sk]");
@@ -948,12 +950,12 @@ std::vector<at::Tensor> evoformer_attention_bwd(const at::Tensor& q, const at::T
   at::Tensor dpair = (has_pb && need_dpair) ? at::zeros({G / groups_per_pair, H, Sq, Sk}, fopt) : at::empty({0}, fopt);
   at::Tensor do_pre = at::empty_like(q), dq_acc = at::empty({G, Sq, H, 32}, fopt);
   const int64_t sq_pad = (Sq + 63) / 64 * 64;
-  at::Tensor lse2 = at::empty({G * H, sq_pad}, fopt), delta = at::empty({G * H, sq_pad}, fopt);
+  at::Tensor m2 = at::empty({G * H, sq_pad}, fopt), delta = at::empty({G * H, sq_pad}, fopt), l2 = at::empty({G * H, sq_pad}, fopt);
   PFX_CUDA_CHECK(pfx::evoformer_attention_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), dout.data_ptr(), has_gate ? gate->data_ptr() : nullptr,
-                                              lse.data_ptr<float>(), has_mb ? mask_bias->data_ptr<float>() : nullptr, has_pb ? pair_bias->data_ptr() : nullptr,
+                                              stats.data_ptr<float>(), has_mb ? mask_bias->data_ptr<float>() : nullptr, has_pb ? pair_bias->data_ptr() : nullptr,
                                               dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), has_gate ? dgate.data_ptr() : nullptr,
                                               dpair.numel() ? dpair.data_ptr<float>() : nullptr, do_pre.data_ptr(), dq_acc.data_ptr<float>(),
-                                              lse2.data_ptr<float>(), delta.data_ptr<float>(), (int)G, (int)Sq, (int)Sk, (int)H, (int)groups_per_pair,
+                                              m2.data_ptr<float>(), delta.data_ptr<float>(), l2.data_ptr<float>(), (int)G, (int)Sq, (int)Sk, (int)H, (int)groups_per_pair,
                                               (float)scale, cur_stream()));
   return {dq, dk, dv, dgate, dpair};
 }

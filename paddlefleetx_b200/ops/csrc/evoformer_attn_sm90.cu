@@ -16,7 +16,9 @@
 //   warp 8    TMA producer: Q tile once per work item, K / V tiles of 128 keys through a 2-stage ring
 //   warps 0-7 two consumer warpgroups (head x = warpgroup): products, biases added on the accumulator fragment (mask bias: one value per
 //             key, pair bias: bf16 pairs of this row), online softmax, P from registers; the epilogue multiplies by sigmoid(gate)
-// Output O (bf16, [g, q, h, 32]) and the row-wise log-sum-exp ([g, h, q] fp32, for the backward).
+// Output O (bf16, [g, q, h, 32]) and, for the backward, the row statistics as two fp32 planes [2, g, h, q]: the row maximum of the logits
+// and log2 of the row sum relative to it, both in log2 units.  They are kept apart because a row whose every key carries the model's
+// -1e9 padding bias has logits near -1.44e9, where the fp32 spacing (128) would absorb log2(Sk) into a single log-sum-exp.
 #include <cstdio>
 
 #include "pfx_ptx.cuh"
@@ -50,7 +52,7 @@ struct EvSmem {
 
 struct EvParams {
   __nv_bfloat16* out;          // [G, Sq, H, 32]
-  float* lse;                  // [G, H, Sq] natural log, or nullptr
+  float* stats;                // [2, G, H, Sq]: row maximum, log2(row sum); log2 units; or nullptr
   const float* mask_bias;      // [G, Sk] fp32 or nullptr
   const __nv_bfloat16* pair_bias;   // [G / groups_per_pair, H, Sq, Sk] bf16 or nullptr
   const __nv_bfloat16* gate;   // [G, Sq, H, 32] pre-sigmoid logits or nullptr
@@ -230,8 +232,11 @@ evoformer_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gr
             }
             *reinterpret_cast<uint32_t*>(prm.out + base + 8 * jj) = pack_bf16x2(v0, v1);
           }
-          if (prm.lse != nullptr && (lane & 3u) == 0)
-            prm.lse[((size_t)g * H + head) * Sq + row_g] = (l_all > 0.f) ? (m_run[hh] + log2f(l_all)) * 0.6931471805599453f : -INFINITY;
+          if (prm.stats != nullptr && (lane & 3u) == 0) {
+            const size_t si = ((size_t)g * H + head) * Sq + row_g;
+            prm.stats[si] = m_run[hh];
+            prm.stats[(size_t)prm.G * H * Sq + si] = (l_all > 0.f) ? log2f(l_all) : -INFINITY;
+          }
         }
       }
     }
@@ -243,7 +248,7 @@ evoformer_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gr
 // the accumulating products from registers, dQ by TMA reduce-add), specialised for a 32-wide head: one CTA = (group, head, 64-key
 // tile); the [.. x 64] TMA tiles carry the head PAIR, the two wgmma K-steps of this head select its half for S^T / dP^T, the N = 64
 // products (dV, dK, dQ) compute the other head's columns as a by-product that is never read.
-//   logits^T = scale K Q^T + mask_bias[k] + pair_bias[q, k]      P^T = exp2(logits^T log2e - lse2[q])
+//   logits^T = scale K Q^T + mask_bias[k] + pair_bias[q, k]      P^T = exp2((logits^T log2e - m2[q]) - l2[q])   (row max, log2 row sum)
 //   dV  += P^T dO'                 dO' = dOut * sigmoid(gate)   (written once by the prep kernel, with dGate and delta = rowsum(dOut o out))
 //   dS^T = P^T o (dP^T - delta[q])      dP^T = V dO'^T
 //   dK  += scale dS^T Q      dQ = scale dS K      dPairBias[q, k] += dS (fp32 red.add: the groups that share a pair bias collide here)
@@ -254,7 +259,7 @@ struct EbSmem {
   static constexpr int kKBytes = kEbKv * kEvD * 2;          //  8 KB: K / V tile of the head pair
   static constexpr int kQBytes = kEbQt * kEvD * 2;          //  8 KB: Q / dO' tile
   static constexpr int kDsBytes = kEbKv * kEbQt * 2;        //  8 KB
-  static constexpr int kStatBytes = 2 * kEbQt * 4;
+  static constexpr int kStatBytes = 3 * kEbQt * 4;          // m2, delta, l2 of one query tile
   static constexpr int kStages = 3;
   static constexpr int kDqBytes = kEbQt * kEvHead * 4;      //  8 KB: dQ tile [64 q][32 d] fp32
   static constexpr int kOffK = 0;
@@ -269,8 +274,9 @@ struct EbSmem {
 };
 
 struct EbParams {
-  const float* lse2;                 // [G*H, Sq_pad] log2 units, +inf in the padding
+  const float* m2;                   // [G*H, Sq_pad] row maximum, log2 units; +inf in the padding and on rows with no finite logit
   const float* delta;                // [G*H, Sq_pad]
+  const float* l2;                   // [G*H, Sq_pad] log2 of the row sum relative to m2; 0 where m2 = +inf
   const float* mask_bias;            // [G, Sk] or null
   const __nv_bfloat16* pair_bias;    // [G / gpp, H, Sq, Sk] or null
   float* dpair;                      // fp32 [G / gpp, H, Sq, Sk] or null
@@ -325,8 +331,9 @@ evoformer_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gr
         tma_load_3d(&tmap_q, q_full(st), s_q + st * S::kQBytes, col, q0, g);
         tma_load_3d(&tmap_do, q_full(st), s_do + st * S::kQBytes, col, q0, g);
         const size_t so = (size_t)gh * prm.Sq_pad + q0;
-        bulk_load_1d(s_stat + st * S::kStatBytes, prm.lse2 + so, kEbQt * 4, q_full(st));
+        bulk_load_1d(s_stat + st * S::kStatBytes, prm.m2 + so, kEbQt * 4, q_full(st));
         bulk_load_1d(s_stat + st * S::kStatBytes + kEbQt * 4, prm.delta + so, kEbQt * 4, q_full(st));
+        bulk_load_1d(s_stat + st * S::kStatBytes + 2 * kEbQt * 4, prm.l2 + so, kEbQt * 4, q_full(st));
       }
     }
   } else {
@@ -368,13 +375,15 @@ evoformer_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gr
       }
       wgmma_commit();
       wgmma_wait<0>();
-      const float* lse_s = reinterpret_cast<const float*>(smem_gen + (s_stat - smem_base) + st * S::kStatBytes);
-      const float* dl_s = lse_s + kEbQt;
+      const float* m_s = reinterpret_cast<const float*>(smem_gen + (s_stat - smem_base) + st * S::kStatBytes);
+      const float* dl_s = m_s + kEbQt;
+      const float* l2_s = m_s + 2 * kEbQt;
       uint32_t pw[kEbQt / 4], dsw[kEbQt / 4];
 #pragma unroll
       for (int gi = 0; gi < kEbQt / 8; ++gi) {
         const int qc = 8 * gi + col_in8;
-        const float2 ls = *reinterpret_cast<const float2*>(lse_s + qc), dl = *reinterpret_cast<const float2*>(dl_s + qc);
+        const float2 mr = *reinterpret_cast<const float2*>(m_s + qc), dl = *reinterpret_cast<const float2*>(dl_s + qc);
+        const float2 l2 = *reinterpret_cast<const float2*>(l2_s + qc);
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
           const int kg = k0 + k_row + 8 * hh;
@@ -384,8 +393,9 @@ evoformer_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gr
             b0 = fmaf(__bfloat162float(prm.pair_bias[(pair_base + min(q0 + qc, prm.Sq - 1)) * prm.Sk + kc[hh]]), kLog2e, b0);
             b1 = fmaf(__bfloat162float(prm.pair_bias[(pair_base + min(q0 + qc + 1, prm.Sq - 1)) * prm.Sk + kc[hh]]), kLog2e, b1);
           }
-          float p0 = exp2f(fmaf(s[4 * gi + 2 * hh], prm.scale_log2, b0) - ls.x);      // lse2 = +inf past Sq -> 0
-          float p1 = exp2f(fmaf(s[4 * gi + 2 * hh + 1], prm.scale_log2, b1) - ls.y);
+          // the logit minus the row maximum first: exact for the -1e9-masked rows, whose logits are all the same fp32 number
+          float p0 = exp2f((fmaf(s[4 * gi + 2 * hh], prm.scale_log2, b0) - mr.x) - l2.x);      // m2 = +inf past Sq -> 0
+          float p1 = exp2f((fmaf(s[4 * gi + 2 * hh + 1], prm.scale_log2, b1) - mr.y) - l2.y);
           if (!k_valid) { p0 = 0.f; p1 = 0.f; }
           pw[2 * gi + hh] = pack_bf16x2(p0, p1);
           const float ds0 = p0 * (dp[4 * gi + 2 * hh] - dl.x), ds1 = p1 * (dp[4 * gi + 2 * hh + 1] - dl.y);
@@ -460,10 +470,10 @@ evoformer_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gr
   }
 }
 
-// prep: dO' = dOut * sigmoid(gate) (bf16), dGate = dOut * out * (1 - sigmoid(gate)), delta = rowsum(dOut o out), lse -> log2 units (padded)
+// prep: dO' = dOut * sigmoid(gate) (bf16), dGate = dOut * out * (1 - sigmoid(gate)), delta = rowsum(dOut o out), row statistics padded
 __global__ void evoformer_bwd_prep_kernel(const __nv_bfloat16* __restrict__ out, const __nv_bfloat16* __restrict__ dout, const __nv_bfloat16* __restrict__ gate,
-                                          const float* __restrict__ lse, __nv_bfloat16* __restrict__ do_pre, __nv_bfloat16* __restrict__ dgate,
-                                          float* __restrict__ lse2, float* __restrict__ delta, int G, int Sq, int H, int Sq_pad) {
+                                          const float* __restrict__ stats, __nv_bfloat16* __restrict__ do_pre, __nv_bfloat16* __restrict__ dgate,
+                                          float* __restrict__ m2, float* __restrict__ delta, float* __restrict__ l2, int G, int Sq, int H, int Sq_pad) {
   const int64_t w = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);      // (g, s_pad, h)
   const int lane = threadIdx.x & 31;
   if (w >= (int64_t)G * Sq_pad * H) return;
@@ -472,7 +482,7 @@ __global__ void evoformer_bwd_prep_kernel(const __nv_bfloat16* __restrict__ out,
   const int g = (int)(w / ((int64_t)H * Sq_pad));
   const size_t oi = ((size_t)g * H + h) * Sq_pad + s;
   if (s >= Sq) {
-    if (lane == 0) { lse2[oi] = INFINITY; delta[oi] = 0.f; }
+    if (lane == 0) { m2[oi] = INFINITY; delta[oi] = 0.f; l2[oi] = 0.f; }
     return;
   }
   const size_t e = (((size_t)g * Sq + s) * H + h) * kEvHead + lane;
@@ -486,7 +496,10 @@ __global__ void evoformer_bwd_prep_kernel(const __nv_bfloat16* __restrict__ out,
   const float acc = warp_sum(d * o);
   if (lane == 0) {
     delta[oi] = acc;
-    lse2[oi] = lse[((size_t)g * H + h) * Sq + s] * 1.4426950408889634f;
+    const size_t si = ((size_t)g * H + h) * Sq + s;
+    const float m = stats[si];
+    m2[oi] = (m == -INFINITY) ? INFINITY : m;             // a row with no finite logit gets P = 0
+    l2[oi] = (m == -INFINITY) ? 0.f : stats[(size_t)G * H * Sq + si];
   }
 }
 
@@ -502,8 +515,8 @@ __global__ void evoformer_f32_to_bf16_kernel(const float* __restrict__ src, __nv
 }  // namespace
 
 // q [G, Sq, H, 32], k / v [G, Sk, H, 32], out [G, Sq, H, 32] bf16 contiguous; mask_bias [G, Sk] fp32 (or null); pair_bias [G / groups_per_pair,
-// H, Sq, Sk] bf16 (or null); gate [G, Sq, H, 32] bf16 pre-sigmoid (or null); lse [G, H, Sq] fp32 (or null).  H even.
-cudaError_t evoformer_attention_fwd(const void* q, const void* k, const void* v, void* out, float* lse, const float* mask_bias, const void* pair_bias,
+// H, Sq, Sk] bf16 (or null); gate [G, Sq, H, 32] bf16 pre-sigmoid (or null); stats [2, G, H, Sq] fp32 (or null).  H even.
+cudaError_t evoformer_attention_fwd(const void* q, const void* k, const void* v, void* out, float* stats, const float* mask_bias, const void* pair_bias,
                                     const void* gate, int G, int Sq, int Sk, int H, int groups_per_pair, float scale, cudaStream_t st) {
   if (G < 1 || Sq < 1 || Sk < 1 || H < 2 || (H & 1) || groups_per_pair < 1 || G % groups_per_pair) return cudaErrorInvalidValue;
   for (const void* p : {q, k, v, (const void*)out})
@@ -533,18 +546,18 @@ cudaError_t evoformer_attention_fwd(const void* q, const void* k, const void* v,
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, evoformer_attn_fwd_kernel, kEvThreads, S::kTotal) != cudaSuccess || per_sm < 1) per_sm = 1;
   const int grid = (int)(items < (long)per_sm * sms ? items : (long)per_sm * sms);
   EvParams prm{};
-  prm.out = (__nv_bfloat16*)out; prm.lse = lse; prm.mask_bias = mask_bias; prm.pair_bias = (const __nv_bfloat16*)pair_bias;
+  prm.out = (__nv_bfloat16*)out; prm.stats = stats; prm.mask_bias = mask_bias; prm.pair_bias = (const __nv_bfloat16*)pair_bias;
   prm.gate = (const __nv_bfloat16*)gate; prm.G = G; prm.Sq = Sq; prm.Sk = Sk; prm.H = H; prm.groups_per_pair = groups_per_pair;
   prm.scale_log2 = scale * 1.4426950408889634f;
   evoformer_attn_fwd_kernel<<<grid, kEvThreads, S::kTotal, st>>>(tq, tk, tv, prm);
   return cudaGetLastError();
 }
 
-// Backward.  Workspaces: do_pre bf16 like q, dq_acc fp32 [G, Sq, H, 32], lse2 / delta fp32 [G*H, round_up(Sq, 64)].  dpair (fp32, zeroed by
+// Backward.  Workspaces: do_pre bf16 like q, dq_acc fp32 [G, Sq, H, 32], m2 / delta / l2 fp32 [G*H, round_up(Sq, 64)].  dpair (fp32, zeroed by
 // the caller) accumulates the pair-bias gradient over the groups; dgate is written only when gate != null.
-cudaError_t evoformer_attention_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout, const void* gate, const float* lse,
+cudaError_t evoformer_attention_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout, const void* gate, const float* stats,
                                     const float* mask_bias, const void* pair_bias, void* dq, void* dk, void* dv, void* dgate, float* dpair,
-                                    void* do_pre, float* dq_acc, float* lse2, float* delta, int G, int Sq, int Sk, int H, int groups_per_pair,
+                                    void* do_pre, float* dq_acc, float* m2, float* delta, float* l2, int G, int Sq, int Sk, int H, int groups_per_pair,
                                     float scale, cudaStream_t st) {
   if (G < 1 || Sq < 1 || Sk < 1 || H < 2 || (H & 1) || groups_per_pair < 1 || G % groups_per_pair) return cudaErrorInvalidValue;
   using S = EbSmem;
@@ -554,8 +567,8 @@ cudaError_t evoformer_attention_bwd(const void* q, const void* k, const void* v,
   if (e != cudaSuccess) return e;
   {
     const int64_t warps = (int64_t)G * Sq_pad * H;
-    evoformer_bwd_prep_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>((const __nv_bfloat16*)out, (const __nv_bfloat16*)dout, (const __nv_bfloat16*)gate, lse,
-                                                                           (__nv_bfloat16*)do_pre, (__nv_bfloat16*)dgate, lse2, delta, G, Sq, H, Sq_pad);
+    evoformer_bwd_prep_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>((const __nv_bfloat16*)out, (const __nv_bfloat16*)dout, (const __nv_bfloat16*)gate, stats,
+                                                                           (__nv_bfloat16*)do_pre, (__nv_bfloat16*)dgate, m2, delta, l2, G, Sq, H, Sq_pad);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
   }
   CUtensorMap tq, tk, tv, tdo, tdq;
@@ -567,7 +580,7 @@ cudaError_t evoformer_attention_bwd(const void* q, const void* k, const void* v,
   ok &= make_tmap_2d_plain(&tdq, dq_acc, 3, row, (uint64_t)G * Sq, row * 4, kEvHead, kEbQt);
   if (!ok) return cudaErrorInvalidValue;
   EbParams prm{};
-  prm.lse2 = lse2; prm.delta = delta; prm.mask_bias = mask_bias; prm.pair_bias = (const __nv_bfloat16*)pair_bias; prm.dpair = dpair;
+  prm.m2 = m2; prm.delta = delta; prm.l2 = l2; prm.mask_bias = mask_bias; prm.pair_bias = (const __nv_bfloat16*)pair_bias; prm.dpair = dpair;
   prm.dk = (__nv_bfloat16*)dk; prm.dv = (__nv_bfloat16*)dv;
   prm.G = G; prm.Sq = Sq; prm.Sk = Sk; prm.H = H; prm.Sq_pad = Sq_pad; prm.gpp = groups_per_pair;
   prm.scale = scale; prm.scale_log2 = scale * 1.4426950408889634f;

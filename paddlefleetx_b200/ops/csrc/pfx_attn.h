@@ -37,15 +37,16 @@ cudaError_t attention_bwd(const AttnView& q, const AttnView& k, const AttnView& 
                           int Sk, int H, int Hkv, int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st);
 
 // Evoformer gated attention (head width 32, H even): softmax(scale QK^T + mask_bias[g, k] + pair_bias[g / groups_per_pair, h, q, k]) V * sigmoid(gate).
-// q / out / gate [G, Sq, H, 32], k / v [G, Sk, H, 32] bf16 contiguous; mask_bias fp32 [G, Sk]; pair_bias bf16; lse fp32 [G, H, Sq].
-cudaError_t evoformer_attention_fwd(const void* q, const void* k, const void* v, void* out, float* lse, const float* mask_bias, const void* pair_bias,
+// q / out / gate [G, Sq, H, 32], k / v [G, Sk, H, 32] bf16 contiguous; mask_bias fp32 [G, Sk]; pair_bias bf16; stats fp32 [2, G, H, Sq]: the
+// row maximum of the logits and log2 of the row sum relative to it (log2 units; log-sum-exp = (stats[0] + stats[1]) ln 2).
+cudaError_t evoformer_attention_fwd(const void* q, const void* k, const void* v, void* out, float* stats, const float* mask_bias, const void* pair_bias,
                                     const void* gate, int G, int Sq, int Sk, int H, int groups_per_pair, float scale, cudaStream_t st);
 
-// Backward of the above.  do_pre (bf16 like q), dq_acc (fp32 like q), lse2 / delta (fp32 [G*H, round_up(Sq, 64)]) are workspaces; dpair is an
-// fp32 accumulator [G / groups_per_pair, H, Sq, Sk] zeroed by the caller (null = no pair-bias gradient); dgate may be null when gate is.
-cudaError_t evoformer_attention_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout, const void* gate, const float* lse,
+// Backward of the above.  do_pre (bf16 like q), dq_acc (fp32 like q), m2 / delta / l2 (fp32 [G*H, round_up(Sq, 64)]) are workspaces; dpair is
+// an fp32 accumulator [G / groups_per_pair, H, Sq, Sk] zeroed by the caller (null = no pair-bias gradient); dgate may be null when gate is.
+cudaError_t evoformer_attention_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout, const void* gate, const float* stats,
                                     const float* mask_bias, const void* pair_bias, void* dq, void* dk, void* dv, void* dgate, float* dpair,
-                                    void* do_pre, float* dq_acc, float* lse2, float* delta, int G, int Sq, int Sk, int H, int groups_per_pair,
+                                    void* do_pre, float* dq_acc, float* m2, float* delta, float* l2, int G, int Sq, int Sk, int H, int groups_per_pair,
                                     float scale, cudaStream_t st);
 
 }  // namespace pfx

@@ -3,8 +3,9 @@
     out[g, q, h, :] = softmax_k(scale * q.k + mask_bias[g, k] + pair_bias[g // groups_per_pair, h, q, k]) @ v * sigmoid(gate)
 
 Forward: one wgmma kernel (``csrc/evoformer_attn_sm90.cu``) — logits, both biases, softmax, P V and the gate never leave the chip; only the
-output and the row-wise log-sum-exp are written.  Backward: a second wgmma kernel recomputes the probabilities per tile from (q, k, biases,
-lse) and produces dq / dk / dv / dgate and the pair-bias gradient (fp32 reductions over the groups that share a bias); nothing of size
+output and two row statistics (the row maximum and log2 of the row sum, kept apart so that rows whose keys all carry the -1e9 padding bias
+keep their 1 / Sk probabilities) are written.  Backward: a second wgmma kernel recomputes the probabilities per tile from (q, k, biases,
+statistics) and produces dq / dk / dv / dgate and the pair-bias gradient (fp32 reductions over the groups that share a bias); nothing of size
 [g, h, q, k] is ever stored (the reference keeps logits, probabilities and the gated average of all 48 blocks x 6 attentions alive).
 ``PFX_EVO_BWD=torch`` selects the older chunked recomputation with library matmuls (also used when the mask bias needs a gradient).
 
@@ -52,9 +53,9 @@ class _EvoAttnFn(torch.autograd.Function):
         mb = None if mask_bias is None else mask_bias.float().contiguous()
         pb = None if pair_bias is None else pair_bias.to(torch.bfloat16).contiguous()
         gt = None if gate is None else gate.contiguous()
-        out, lse = lib.evoformer_attention_fwd(q, k, v, mb, pb, gt, groups_per_pair, scale)
+        out, stats = lib.evoformer_attention_fwd(q, k, v, mb, pb, gt, groups_per_pair, scale)
         ctx.save_for_backward(q, k, v, mb if mb is not None else q.new_empty(0), pb if pb is not None else q.new_empty(0),
-                              gt if gt is not None else q.new_empty(0), lse, out)
+                              gt if gt is not None else q.new_empty(0), stats, out)
         ctx.flags = (mask_bias is not None, pair_bias is not None, gate is not None)
         ctx.gpp, ctx.scale = groups_per_pair, scale
         ctx.bias_dtypes = (None if mask_bias is None else mask_bias.dtype, None if pair_bias is None else pair_bias.dtype)
@@ -63,9 +64,9 @@ class _EvoAttnFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dout):
         """Gradients of the gated attention w.r.t. q / k / v, the two additive biases and the gate: the native kernel recomputes the probabilities
-        from the saved log-sum-exp tile by tile (dK / dV in tensor memory, dQ through an fp32 workspace); bias gradients are reduced over the axes
+        from the saved row statistics tile by tile (dK / dV in tensor memory, dQ through an fp32 workspace); bias gradients are reduced over the axes
         the biases were broadcast along."""
-        q, k, v, mb, pb, gt, lse = ctx.saved_tensors[:7]
+        q, k, v, mb, pb, gt, stats = ctx.saved_tensors[:7]
         has_mb, has_pb, has_gate = ctx.flags
         gpp, scale = ctx.gpp, ctx.scale
         G, Sq, H, D = q.shape
@@ -77,7 +78,7 @@ class _EvoAttnFn(torch.autograd.Function):
             lib = _native.require()
             out = ctx.saved_tensors[7]
             need_pb = has_pb and ctx.needs_input_grad[4]
-            dq, dk, dv, dgate, dpair = lib.evoformer_attention_bwd(q, k, v, out, dout, lse, mb if has_mb else None, pb if has_pb else None,
+            dq, dk, dv, dgate, dpair = lib.evoformer_attention_bwd(q, k, v, out, dout, stats, mb if has_mb else None, pb if has_pb else None,
                                                                    gt if has_gate else None, gpp, scale, need_pb)
             mb_dt, pb_dt = ctx.bias_dtypes
             return (dq, dk, dv, None, dpair.to(pb_dt) if need_pb else None, dgate if has_gate else None, None, None)
@@ -98,13 +99,16 @@ class _EvoAttnFn(torch.autograd.Function):
             g1 = min(g0 + step, G)
             sl = slice(g0, g1)
             qc, kc, vc = q[sl], k[sl], v[sl]
-            logits = torch.einsum("gqhd,gkhd->ghqk", qc, kc).float() * scale
+            # fp32 products: a 16-bit q.k rounds every logit by 2^-8 relative, which exp() turns into a probability error of about 1 %
+            logits = torch.einsum("gqhd,gkhd->ghqk", qc.float(), kc.float()) * scale
             if has_mb:
                 logits += mb[sl].view(g1 - g0, 1, 1, Sk)
             if has_pb:
                 idx = torch.arange(g0, g1, device=q.device) // gpp
                 logits += pb.index_select(0, idx).float()
-            p = torch.exp(logits - lse[sl].unsqueeze(-1))                       # [g, h, q, k] fp32, rows sum to 1
+            # softmax of the recomputed logits, not exp(logits - lse): on a row whose keys all carry -1e9 the fp32 logits are all equal and
+            # their log-sum-exp loses log(Sk) to rounding
+            p = torch.softmax(logits, -1)                                       # [g, h, q, k] fp32, rows sum to 1
             del logits
             pb16 = p.to(q.dtype)                                                # matmul operands in the activations' dtype
             do = dout[sl]

@@ -15,9 +15,8 @@ pytestmark = pytest.mark.gpu
 
 F16, B16 = torch.float16, torch.bfloat16
 EPI_NONE, EPI_BIAS, EPI_BIAS_GELU, EPI_GELU = 0, 1, 2, 3
-# In-chain error of the fp32 tensor-core accumulation, relative to the sum of |terms|: the PTX ISA does not document the accumulator's
-# width, so the bound leaves room for a truncating one.  A tile, stage or staging buffer mixed up is wrong by the size of the result.
-MMA_ACC = 2.0 ** -16
+# A tile, stage or staging buffer mixed up is wrong by the size of the result, far outside the R.MMA_ACC allowance.
+MMA_ACC = R.MMA_ACC
 
 
 @pytest.fixture(scope="module")
