@@ -17,6 +17,9 @@ The fused-QKV output dimension is laid out ``[heads, 3, head_dim]`` like the ref
 (``num_key_value_heads`` = Hkv < heads, G = heads / Hkv query heads per K/V head) it is ``[Hkv, G + 2, head_dim]``: the G query heads of
 a group, then its key, then its value.  G = 1 is the ``[heads, 3, head_dim]`` layout, and because the layout splits by whole groups
 along the output rows, tensor parallelism shards it like any column-parallel weight when ``Hkv % mp == 0``.
+With ``ffn_activation="swiglu"`` the FFN is h = silu(x W_g + b_g) * (x W_u + b_u) of width F = ``ffn_hidden_size``, and ``linear1`` is
+``[2F, H]`` with pair-interleaved rows: row 2i is gate channel i, row 2i + 1 its up channel (the bias likewise).  A contiguous
+column-parallel shard then holds whole pairs, so tensor parallelism and checkpoint resharding split ``linear1`` as before.
 """
 from __future__ import annotations
 
@@ -72,6 +75,15 @@ class RMSNorm(nn.Module):
 
     def forward_res(self, x):
         return OF.norm_with_residual(x, self.weight, None, self.eps, True)
+
+
+FFN_ACTIVATIONS = ("gelu", "swiglu")
+
+
+def swiglu_ffn_size(hidden: int) -> int:
+    """Default SwiGLU width: 8h/3 rounded up to a multiple of 256 (5632 at h = 2048), which keeps the FFN's parameter count near that of
+    a 4h GELU FFN."""
+    return -(-8 * hidden // (3 * 256)) * 256
 
 
 def make_norm(kind: Optional[str], hidden: int, sequence_parallel: bool = False, dtype=None, device=None) -> nn.Module:
@@ -301,8 +313,14 @@ class TransformerDecoderLayer(nn.Module):
     def __init__(self, hidden: int, num_heads: int, ffn_hidden: int, hidden_dropout: float = 0.1, attn_dropout: float = 0.1,
                  num_layers: int = 1, sequence_parallel: bool = False, mp_group=None, init_std: float = 0.02,
                  recompute_attn: bool = False, recompute_core: bool = False, moe_layer: Optional[nn.Module] = None,
-                 fused_tp_comm: bool = False, normalization: Optional[str] = None, dtype=None, device=None, **attn_kwargs):
+                 fused_tp_comm: bool = False, normalization: Optional[str] = None, ffn_activation: str = "gelu", dtype=None, device=None,
+                 **attn_kwargs):
         super().__init__()
+        if ffn_activation not in FFN_ACTIVATIONS:
+            raise ValueError(f"Model.ffn_activation must be one of {', '.join(FFN_ACTIVATIONS)}, got {ffn_activation!r}")
+        if ffn_activation == "swiglu" and moe_layer is not None:
+            raise ValueError("ffn_activation: swiglu is not supported with MoE layers (moe_configs); the experts keep GELU")
+        self.ffn_activation = ffn_activation
         out_std = init_std / math.sqrt(2.0 * num_layers)
         self.sequence_parallel = sequence_parallel
         self.hidden_dropout = hidden_dropout
@@ -318,7 +336,8 @@ class TransformerDecoderLayer(nn.Module):
             Row = RowSequenceParallelLinear if sequence_parallel else RowParallelLinear
             kw = dict(mp_group=mp_group, dtype=dtype, device=device)
             extra = dict(fused_comm=fused_tp_comm) if sequence_parallel else {}
-            self.linear1 = Col(hidden, ffn_hidden, gather_output=False, init_std=init_std, has_bias=True, **kw, **extra)
+            ffn1_width = 2 * ffn_hidden if ffn_activation == "swiglu" else ffn_hidden      # gate / up pairs, interleaved
+            self.linear1 = Col(hidden, ffn1_width, gather_output=False, init_std=init_std, has_bias=True, **kw, **extra)
             self.linear2 = Row(ffn_hidden, hidden, input_is_parallel=True, init_std=out_std, skip_bias_add=True, **kw, **extra)
         # hidden dropout stream: identical inside the TP group without SP, distinct under SP
         self.rng_name = "local_seed" if sequence_parallel else "global_seed"
@@ -330,6 +349,8 @@ class TransformerDecoderLayer(nn.Module):
 
     def _ffn(self, h):
         l1, l2 = self.linear1, self.linear2
+        if self.ffn_activation == "swiglu":
+            return l2(OF.bias_swiglu(l1(h, skip_bias=True), l1.bias))
         if (getattr(l1, "world", 1) == 1 and not self.self_attn.sequence_parallel and getattr(l1, "int8", None) is None and l1.weight is not None
                 and not getattr(l1, "needs_forward", False) and not getattr(l2, "needs_forward", False)
                 and l1.bias is not None and getattr(l2, "skip_bias_add", False) and not _TP_OPTIONS["fp8_tp_gemm"]):
@@ -352,7 +373,7 @@ class TransformerDecoderLayer(nn.Module):
 
     def _decode_fast(self, x, attn_mask, cache):
         """One decode token through the layer in five launches: LN1+QKV GEMV, cache-append + attention, out-proj GEMV + bias + residual,
-        LN2+FFN1 GEMV + bias + GELU, FFN2 GEMV + bias + residual (the generic path takes thirteen)."""
+        LN2+FFN1 GEMV + bias + GELU / SwiGLU, FFN2 GEMV + bias + residual (the generic path takes thirteen)."""
         a = self.self_attn
         b = x.shape[0]
         x2 = x.reshape(b, -1)
@@ -360,7 +381,8 @@ class TransformerDecoderLayer(nn.Module):
         o = OF.attention_decode_packed(qkv.view(b, 1, a.local_kv_heads, a.group + 2, a.head_dim), cache.k, cache.v, attn_mask, cache.static_index,
                                        1.0 / math.sqrt(a.head_dim))
         x2 = OF.gemv_fused(o.view(b, -1), a.out_proj.weight, a.out_proj.bias, residual=x2)
-        h = OF.gemv_fused(x2, self.linear1.weight, self.linear1.bias, ln=(self.norm2.weight, self.norm2.bias, self.norm2.eps), act="gelu")
+        h = OF.gemv_fused(x2, self.linear1.weight, self.linear1.bias, ln=(self.norm2.weight, self.norm2.bias, self.norm2.eps),
+                          act=self.ffn_activation)
         x2 = OF.gemv_fused(h, self.linear2.weight, self.linear2.bias, residual=x2)
         return x2.view_as(x)
 
@@ -440,9 +462,10 @@ class GPTModel(nn.Module):
                  fused_linear: bool = False, fuse_attn_qkv: bool = True, scale_qk_by_layer_num: bool = True,
                  sequence_parallel: bool = False, use_flash_attn: bool = True, fused_softmax_with_triangular: bool = True,
                  mp_group=None, moe_configs: Optional[dict] = None, fused_tp_comm: bool = False, use_rope: bool = False,
-                 normalization: Optional[str] = None, num_key_value_heads: Optional[int] = None, dtype=None, device=None, **unused):
+                 normalization: Optional[str] = None, num_key_value_heads: Optional[int] = None, ffn_activation: str = "gelu", dtype=None,
+                 device=None, **unused):
         super().__init__()
-        ffn_hidden_size = ffn_hidden_size or 4 * hidden_size
+        ffn_hidden_size = ffn_hidden_size or (swiglu_ffn_size(hidden_size) if ffn_activation == "swiglu" else 4 * hidden_size)
         recompute_granularity = recompute_granularity or "full"
         self.hidden_size, self.vocab_size, self.num_layers = hidden_size, vocab_size, num_layers
         self.initializer_range = initializer_range
@@ -466,7 +489,7 @@ class GPTModel(nn.Module):
                 dtype=dtype, device=device, fuse_attn_qkv=fuse_attn_qkv,
                 scale_qk_coeff=float(num_layers) if scale_qk_by_layer_num else 1.0, use_flash_attn=use_flash_attn,
                 fused_softmax_with_triangular=fused_softmax_with_triangular, use_rope=use_rope, normalization=normalization,
-                num_key_value_heads=num_key_value_heads))
+                num_key_value_heads=num_key_value_heads, ffn_activation=ffn_activation))
         self.decoder = TransformerDecoder(layers, hidden_size, use_recompute, recompute_granularity, no_recompute_layers, sp, dtype, device,
                                           normalization=normalization)
 

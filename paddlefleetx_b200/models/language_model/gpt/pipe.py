@@ -60,8 +60,8 @@ class GPTForPretrainingPipe(PipelineLayer):
                  fuse_attn_qkv: bool = True, scale_qk_by_layer_num: bool = True, sequence_parallel: bool = False,
                  use_flash_attn: bool = True, fused_softmax_with_triangular: bool = True, virtual_pp_degree: int = 1,
                  pp_recompute_interval: int = 1, fused_tp_comm: bool = False, use_rope: bool = False, normalization=None,
-                 num_key_value_heads: Optional[int] = None, dtype=None, device=None, **unused):
-        ffn_hidden_size = ffn_hidden_size or 4 * hidden_size
+                 num_key_value_heads: Optional[int] = None, ffn_activation: str = "gelu", dtype=None, device=None, **unused):
+        ffn_hidden_size = ffn_hidden_size or (gpt.swiglu_ffn_size(hidden_size) if ffn_activation == "swiglu" else 4 * hidden_size)
         recompute_granularity = recompute_granularity or "full"
         sp = sequence_parallel and C.group_size(mp_group) > 1
         embed_args = dict(vocab_size=vocab_size, hidden=hidden_size, max_position=max_position_embeddings,
@@ -76,7 +76,7 @@ class GPTForPretrainingPipe(PipelineLayer):
                 recompute_core=use_recompute and recompute_granularity == "core_attn", fused_tp_comm=fused_tp_comm, dtype=dtype,
                 device=device, fuse_attn_qkv=fuse_attn_qkv, scale_qk_coeff=float(num_layers) if scale_qk_by_layer_num else 1.0,
                 use_flash_attn=use_flash_attn, fused_softmax_with_triangular=fused_softmax_with_triangular, use_rope=use_rope,
-                normalization=normalization, num_key_value_heads=num_key_value_heads))
+                normalization=normalization, num_key_value_heads=num_key_value_heads, ffn_activation=ffn_activation))
         descs.append(LayerDesc(LayerNormPipe, hidden_size, sp, mp_group, dtype, device, normalization))
         descs.append(SharedLayerDesc("embed", EmbeddingPipe, forward_func=_logits_helper, shared_weight_attr="embedding_weight", **embed_args))
         interval = pp_recompute_interval if (use_recompute and recompute_granularity == "full") else 0

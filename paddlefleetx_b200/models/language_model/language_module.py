@@ -50,7 +50,7 @@ def process_data_configs(config) -> None:
 def process_model_configs(config) -> None:
     m = config.Model
     if m.get("ffn_hidden_size") is None:
-        m["ffn_hidden_size"] = 4 * m["hidden_size"]
+        m["ffn_hidden_size"] = gpt.swiglu_ffn_size(m["hidden_size"]) if m.get("ffn_activation") == "swiglu" else 4 * m["hidden_size"]
     if m.get("use_recompute"):
         if not m.get("recompute_granularity"):
             m["recompute_granularity"] = "full"
@@ -103,10 +103,14 @@ def process_configs(config):
     return config
 
 
-def get_model_size(l: int, h: int, v: int, s: int, kv_hidden: Optional[int] = None) -> float:
-    """Parameter count; ``kv_hidden`` = K/V heads x head_dim (grouped-query attention), default ``h``: QKV is h (h + 2 kv_hidden)."""
+def get_model_size(l: int, h: int, v: int, s: int, kv_hidden: Optional[int] = None, ffn: Optional[int] = None,
+                   ffn_activation: str = "gelu") -> float:
+    """Parameter count; ``kv_hidden`` = K/V heads x head_dim (grouped-query attention), default ``h``: QKV is h (h + 2 kv_hidden).  ``ffn``
+    is the FFN width F (default 4h): 2hF + F + h parameters under GELU, 3hF + 2F + h under SwiGLU (``linear1`` is [2F, h])."""
     kv = h if kv_hidden is None else kv_hidden
-    p = (v + s) * h + (2 * h * h + 2 * h * kv + 2 * h + 2 * kv) * l + (2 * (2 * h)) * l + (8 * h * h + 5 * h) * l + 2 * h
+    f = 4 * h if ffn is None else ffn
+    ffn_params = (3 * h * f + 2 * f + h) if ffn_activation == "swiglu" else (2 * h * f + f + h)
+    p = (v + s) * h + (2 * h * h + 2 * h * kv + 2 * h + 2 * kv) * l + (2 * (2 * h)) * l + ffn_params * l + 2 * h
     logger.info("Model Size: {:.2f} B".format(p / 1e9))
     return p
 
@@ -115,7 +119,7 @@ _MODEL_KEYS = ("vocab_size", "hidden_size", "num_layers", "num_attention_heads",
                "attention_probs_dropout_prob", "max_position_embeddings", "type_vocab_size", "initializer_range", "use_recompute",
                "recompute_granularity", "no_recompute_layers", "fused_linear", "fuse_attn_qkv", "scale_qk_by_layer_num",
                "sequence_parallel", "use_flash_attn", "fused_softmax_with_triangular", "moe_configs", "use_rope", "normalization", "virtual_pp_degree",
-               "num_key_value_heads")
+               "num_key_value_heads", "ffn_activation")
 
 
 def model_kwargs(config) -> dict:
@@ -250,7 +254,8 @@ class GPTModule(LanguageModule):
         kw = model_kwargs(cfg)
         kw["vocab_size"] = vocab
         kv_hidden = kw["hidden_size"] // kw["num_attention_heads"] * kw["num_key_value_heads"] if kw.get("num_key_value_heads") else None
-        get_model_size(kw["num_layers"], kw["hidden_size"], vocab, kw.get("max_position_embeddings", 1024), kv_hidden)
+        get_model_size(kw["num_layers"], kw["hidden_size"], vocab, kw.get("max_position_embeddings", 1024), kv_hidden, kw.get("ffn_hidden_size"),
+                       kw.get("ffn_activation", "gelu"))
         dtype, device = _param_dtype(cfg), _device(cfg)
         fused_tp = bool(cfg.get("Fused", {}).get("tp_comm", False))
         if d.pp_degree > 1:

@@ -344,6 +344,40 @@ at::Tensor bias_gelu_bwd(const at::Tensor& dy, const at::Tensor& x, c10::optiona
                                 dx.data_ptr(), x.numel() / cols, (int)cols, dtype_code(x), true, num_sms(), cur_stream(), exact));
   return dx;
 }
+// SwiGLU over pair-interleaved z [.., 2F] (column 2i gate channel i, 2i + 1 its up channel) -> h [.., F]
+at::Tensor bias_swiglu_fwd(const at::Tensor& z, c10::optional<at::Tensor> bias) {
+  PFX_CHECK_CUDA_CONTIG(z);
+  check_16bit(z, "bias_swiglu", "z");
+  check_same_dtype(z, bias, "bias_swiglu");
+  const int64_t cols = z.size(-1);
+  TORCH_CHECK(cols % 16 == 0, "bias_swiglu: z needs 2F columns with F % 8 == 0, got ", cols);
+  if (bias.has_value() && bias->defined())
+    TORCH_CHECK(bias->is_contiguous() && bias->numel() == cols, "bias_swiglu: bias has ", bias->numel(), " elements for rows of ", cols);
+  const c10::cuda::CUDAGuard guard(z.device());
+  auto sizes = z.sizes().vec();
+  sizes.back() = cols / 2;
+  auto h = at::empty(sizes, z.options());
+  PFX_CUDA_CHECK(pfx::bias_swiglu(z.data_ptr(), (bias.has_value() && bias->defined()) ? bias->data_ptr() : nullptr, nullptr, h.data_ptr(),
+                                  z.numel() / cols, (int)(cols / 2), dtype_code(z), false, num_sms(), cur_stream()));
+  return h;
+}
+at::Tensor bias_swiglu_bwd(const at::Tensor& dh, const at::Tensor& z, c10::optional<at::Tensor> bias) {
+  PFX_CHECK_CUDA_CONTIG(z); PFX_CHECK_CUDA_CONTIG(dh);
+  check_16bit(z, "bias_swiglu_bwd", "z");
+  check_same_dtype(z, bias, "bias_swiglu_bwd");
+  check_like(dh, z, "bias_swiglu_bwd", "dh");
+  const int64_t cols = z.size(-1);
+  TORCH_CHECK(cols % 16 == 0, "bias_swiglu_bwd: z needs 2F columns with F % 8 == 0, got ", cols);
+  TORCH_CHECK(dh.dim() == z.dim() && dh.size(-1) * 2 == cols && dh.numel() * 2 == z.numel(), "bias_swiglu_bwd: dh ", dh.sizes(),
+              " does not match z ", z.sizes());
+  if (bias.has_value() && bias->defined())
+    TORCH_CHECK(bias->is_contiguous() && bias->numel() == cols, "bias_swiglu_bwd: bias has ", bias->numel(), " elements for rows of ", cols);
+  const c10::cuda::CUDAGuard guard(z.device());
+  auto dz = at::empty_like(z);
+  PFX_CUDA_CHECK(pfx::bias_swiglu(z.data_ptr(), (bias.has_value() && bias->defined()) ? bias->data_ptr() : nullptr, dh.data_ptr(),
+                                  dz.data_ptr(), z.numel() / cols, (int)(cols / 2), dtype_code(z), true, num_sms(), cur_stream()));
+  return dz;
+}
 at::Tensor bias_dropout_add_fwd(const at::Tensor& x, c10::optional<at::Tensor> bias, c10::optional<at::Tensor> residual, double p,
                                 int64_t seed, int64_t offset) {
   PFX_CHECK_CUDA_CONTIG(x);
@@ -655,7 +689,9 @@ at::Tensor gemv_fused(const at::Tensor& x, const at::Tensor& w, c10::optional<at
                       c10::optional<at::Tensor> ln_b, double ln_eps, c10::optional<at::Tensor> residual, int64_t act) {
   TORCH_CHECK(x.is_cuda() && x.dim() == 2 && w.dim() == 2 && x.is_contiguous() && w.is_contiguous() && x.size(1) == w.size(1), "gemv_fused: x [M,K], w [N,K]");
   TORCH_CHECK(x.scalar_type() == w.scalar_type(), "gemv_fused: dtype mismatch");
-  at::Tensor y = at::empty({x.size(0), w.size(0)}, x.options());
+  TORCH_CHECK(act >= 0 && act <= 2, "gemv_fused: act must be 0 (none), 1 (GELU) or 2 (SwiGLU), got ", act);
+  TORCH_CHECK(act != 2 || w.size(0) % 2 == 0, "gemv_fused: SwiGLU needs an even number of weight rows (gate, up pairs), got ", w.size(0));
+  at::Tensor y = at::empty({x.size(0), act == 2 ? w.size(0) / 2 : w.size(0)}, x.options());
   auto ptr = [](const c10::optional<at::Tensor>& t) -> const void* { return (t.has_value() && t->defined()) ? t->data_ptr() : nullptr; };
   if (residual.has_value() && residual->defined())
     TORCH_CHECK(residual->is_contiguous() && residual->numel() == y.numel() && residual->scalar_type() == x.scalar_type(), "gemv_fused: residual [M,N]");
@@ -1060,6 +1096,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("dres") = py::none());
   m.def("bias_gelu_fwd", &bias_gelu_fwd);
   m.def("bias_gelu_bwd", &bias_gelu_bwd);
+  m.def("bias_swiglu_fwd", &bias_swiglu_fwd);
+  m.def("bias_swiglu_bwd", &bias_swiglu_bwd);
   m.def("bias_dropout_add_fwd", &bias_dropout_add_fwd);
   m.def("dropout_bwd", &dropout_bwd);
   m.def("colsum", &colsum);

@@ -15,22 +15,23 @@ namespace {
 
 // Optional fusions for the decode step (every removed launch is ~5 us of a ~100 us layer): LayerNorm of the activation rows as
 // a prologue (each CTA recomputes the two row statistics from the L1/L2-resident x — K reads against N*K/CTAs weight reads),
-// GELU, and "+ residual" in the finish.
+// GELU or SwiGLU, and "+ residual" in the finish.
 template <typename T>
 struct GemvExtra {
   const T* ln_w = nullptr;       // LayerNorm gamma (null = no norm)
   const T* ln_b = nullptr;
   float ln_eps = 1e-5f;
-  const T* residual = nullptr;   // [M, N] added after bias / activation
-  int act = 0;                   // 0 none, 1 GELU(tanh)
+  const T* residual = nullptr;   // [M, N] ([M, N / 2] under SwiGLU) added after bias / activation
+  int act = 0;                   // 0 none, 1 GELU(tanh), 2 SwiGLU over pair-interleaved rows: y[r, n / 2] = silu(v[r, n]) v[r, n + 1]
 };
 
 __device__ __forceinline__ float gemv_gelu_tanh(float x) {
   return 0.5f * x * (1.f + tanhf(0.7978845608028654f * (x + 0.044715f * x * x * x)));
 }
 
-// block = 8 warps arranged as (8 / kSplit) column groups x kSplit K-slices; a column group owns kCols weight rows.
-template <typename T, int kRows, int kCols, int kSplit>
+// block = 8 warps arranged as (8 / kSplit) column groups x kSplit K-slices; a column group owns kCols weight rows.  kSwiglu selects the
+// SwiGLU finish (act 2) at compile time, so that the other instantiations keep their code and registers.
+template <typename T, int kRows, int kCols, int kSplit, bool kSwiglu>
 __global__ void __launch_bounds__(256) gemv_skinny_kernel(const T* __restrict__ x, const T* __restrict__ w, const T* __restrict__ bias,
                                                           T* __restrict__ y, int N, int K, const GemvExtra<T> ex) {
   constexpr int kGroups = 8 / kSplit;
@@ -127,17 +128,33 @@ __global__ void __launch_bounds__(256) gemv_skinny_kernel(const T* __restrict__ 
       if (lane == 0) red[wid][c * kRows + r] = v;
     }
   __syncthreads();
-  // one thread per (group, column, row) finishes the K-slice sum and writes the output
-  for (int t = threadIdx.x; t < kGroups * kCols * kRows; t += blockDim.x) {
-    const int g = t / (kCols * kRows), cr = t % (kCols * kRows), c = cr / kRows, r = cr % kRows;
-    const int n = (blockIdx.x * kGroups + g) * kCols + c;
-    if (n >= N) continue;
-    float v = bias ? to_f32<T>(bias[n]) : 0.f;
+  if constexpr (kSwiglu) {
+    // SwiGLU: a column group starts on an even weight row, so each of its column pairs (gate, up) is finished by one thread
+    const int N2 = N >> 1;
+    for (int t = threadIdx.x; t < kGroups * (kCols / 2) * kRows; t += blockDim.x) {
+      const int g = t / ((kCols / 2) * kRows), pr = t % ((kCols / 2) * kRows), c = 2 * (pr / kRows), r = pr % kRows;
+      const int n = (blockIdx.x * kGroups + g) * kCols + c;
+      if (n >= N) continue;
+      float a = bias ? to_f32<T>(bias[n]) : 0.f, b = bias ? to_f32<T>(bias[n + 1]) : 0.f;
 #pragma unroll
-    for (int s2 = 0; s2 < kSplit; ++s2) v += red[g * kSplit + s2][cr];
-    if (ex.act == 1) v = gemv_gelu_tanh(v);
-    if (ex.residual != nullptr) v += to_f32<T>(ex.residual[(size_t)r * N + n]);
-    y[(size_t)r * N + n] = from_f32<T>(v);
+      for (int s2 = 0; s2 < kSplit; ++s2) { a += red[g * kSplit + s2][c * kRows + r]; b += red[g * kSplit + s2][(c + 1) * kRows + r]; }
+      float v = a * (1.f / (1.f + __expf(-a))) * b;              // the form of bias_swiglu_kernel (norm_act.cu)
+      if (ex.residual != nullptr) v += to_f32<T>(ex.residual[(size_t)r * N2 + (n >> 1)]);
+      y[(size_t)r * N2 + (n >> 1)] = from_f32<T>(v);
+    }
+  } else {
+    // one thread per (group, column, row) finishes the K-slice sum and writes the output
+    for (int t = threadIdx.x; t < kGroups * kCols * kRows; t += blockDim.x) {
+      const int g = t / (kCols * kRows), cr = t % (kCols * kRows), c = cr / kRows, r = cr % kRows;
+      const int n = (blockIdx.x * kGroups + g) * kCols + c;
+      if (n >= N) continue;
+      float v = bias ? to_f32<T>(bias[n]) : 0.f;
+#pragma unroll
+      for (int s2 = 0; s2 < kSplit; ++s2) v += red[g * kSplit + s2][cr];
+      if (ex.act == 1) v = gemv_gelu_tanh(v);
+      if (ex.residual != nullptr) v += to_f32<T>(ex.residual[(size_t)r * N + n]);
+      y[(size_t)r * N + n] = from_f32<T>(v);
+    }
   }
 }
 
@@ -145,7 +162,8 @@ template <typename T, int kRows, int kCols, int kSplit>
 cudaError_t launch_cfg(const T* x, const T* w, const T* bias, T* y, int N, int K, const GemvExtra<T>& ex, cudaStream_t st) {
   constexpr int kGroups = 8 / kSplit;
   const int groups = (N + kCols - 1) / kCols;
-  gemv_skinny_kernel<T, kRows, kCols, kSplit><<<(groups + kGroups - 1) / kGroups, 256, 0, st>>>(x, w, bias, y, N, K, ex);
+  if (ex.act == 2) gemv_skinny_kernel<T, kRows, kCols, kSplit, true><<<(groups + kGroups - 1) / kGroups, 256, 0, st>>>(x, w, bias, y, N, K, ex);
+  else gemv_skinny_kernel<T, kRows, kCols, kSplit, false><<<(groups + kGroups - 1) / kGroups, 256, 0, st>>>(x, w, bias, y, N, K, ex);
   return cudaGetLastError();
 }
 
@@ -300,7 +318,7 @@ cudaError_t launch(const void* x, const void* w, const void* bias, void* y, int 
 
 cudaError_t gemv_skinny(const void* x, const void* w, const void* bias, void* y, int M, int N, int K, int dtype, int num_sms, cudaStream_t st,
                         const void* ln_w, const void* ln_b, float ln_eps, const void* residual, int act) {
-  if (M < 1 || M > 8 || K % 8 || ((ln_w == nullptr) != (ln_b == nullptr))) return cudaErrorInvalidValue;
+  if (M < 1 || M > 8 || K % 8 || ((ln_w == nullptr) != (ln_b == nullptr)) || (act == 2 && N % 2)) return cudaErrorInvalidValue;
   if (dtype == 1) return launch<__nv_bfloat16>(x, w, bias, y, M, N, K, num_sms, ln_w, ln_b, ln_eps, residual, act, st);
   if (dtype == 0) return launch<__half>(x, w, bias, y, M, N, K, num_sms, ln_w, ln_b, ln_eps, residual, act, st);
   return cudaErrorInvalidValue;

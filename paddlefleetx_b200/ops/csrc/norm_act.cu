@@ -1,4 +1,4 @@
-// Bandwidth-bound fused kernels: LayerNorm / RMSNorm fwd+bwd, bias+GELU fwd+bwd,
+// Bandwidth-bound fused kernels: LayerNorm / RMSNorm fwd+bwd, bias+GELU fwd+bwd, bias+SwiGLU fwd+bwd,
 // bias + Philox-dropout + residual fwd (mask regenerated in bwd, never stored), column sums.
 // Reference call sites: L8 (LayerNorm), L10 (dropout+residual), L3 (GELU) in SURVEY §2.6 — Paddle
 // runs each as a separate library kernel; here every one is a single pass over HBM with 128-bit IO.
@@ -320,6 +320,72 @@ cudaError_t bias_gelu(const void* x, const void* bias, const void* dy, void* out
 #define PFX_LAUNCH(T)                                                                                                     \
   if (bwd) bias_gelu_kernel<T, true><<<grid, threads, 0, st>>>((const T*)x, (const T*)bias, (const T*)dy, (T*)out, total, cols / 8, exact); \
   else bias_gelu_kernel<T, false><<<grid, threads, 0, st>>>((const T*)x, (const T*)bias, nullptr, (T*)out, total, cols / 8, exact);
+  if (dtype == 1) { PFX_LAUNCH(__nv_bfloat16) } else { PFX_LAUNCH(__half) }
+#undef PFX_LAUNCH
+  return cudaGetLastError();
+}
+
+// --------------------------------------------------------------------------- bias + SwiGLU
+// z [rows, 2F] holds pair-interleaved FFN1 outputs: column 2i is gate channel i, column 2i + 1 its up channel, so one thread's 16 z
+// elements (two 16-byte vectors) are the 8 pairs behind one 16-byte vector of h [rows, F].  a = g + b_g, b = u + b_u, s = sigmoid(a):
+//   fwd  h  = a s b
+//   bwd  dg = dh b s (1 + a (1 - s)),   du = dh a s
+// A saturated gate stays finite: __expf(-a) overflows to inf for a < -88, s = 1 / inf = 0 and every product above is 0 (1 - s is formed
+// directly, never as e s, which would be inf * 0).
+__device__ __forceinline__ float swiglu_sigmoid(float a) { return 1.f / (1.f + __expf(-a)); }
+
+template <typename T, bool kBwd>
+__global__ void bias_swiglu_kernel(const T* __restrict__ z, const T* __restrict__ bias, const T* __restrict__ dh, T* __restrict__ out,
+                                   size_t total_vec, int nvec_row) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total_vec; i += (size_t)gridDim.x * blockDim.x) {
+    float zv[2][8];                              // pair j: gate zv[j / 4][2 (j % 4)], up zv[j / 4][2 (j % 4) + 1]
+    const uint4* zp = reinterpret_cast<const uint4*>(z) + 2 * i;
+    unpack8<T>(ld_stream(zp), zv[0]);
+    unpack8<T>(ld_stream(zp + 1), zv[1]);
+    if (bias) {
+      float bv[2][8];
+      const uint4* bp = reinterpret_cast<const uint4*>(bias) + 2 * (i % nvec_row);
+      unpack8<T>(__ldg(bp), bv[0]);
+      unpack8<T>(__ldg(bp + 1), bv[1]);
+#pragma unroll
+      for (int k = 0; k < 2; ++k)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) zv[k][j] += bv[k][j];
+    }
+    if (kBwd) {
+      float gv[8], o[2][8];
+      unpack8<T>(ld_stream(reinterpret_cast<const uint4*>(dh) + i), gv);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int k = j >> 2, c = 2 * (j & 3);
+        const float a = zv[k][c], b = zv[k][c + 1], s = swiglu_sigmoid(a);
+        o[k][c] = gv[j] * b * s * (1.f + a * (1.f - s));
+        o[k][c + 1] = gv[j] * a * s;
+      }
+      uint4* op = reinterpret_cast<uint4*>(out) + 2 * i;
+      st_stream(op, pack8<T>(o[0]));
+      st_stream(op + 1, pack8<T>(o[1]));
+    } else {
+      float o[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int k = j >> 2, c = 2 * (j & 3);
+        o[j] = zv[k][c] * swiglu_sigmoid(zv[k][c]) * zv[k][c + 1];
+      }
+      st_stream(reinterpret_cast<uint4*>(out) + i, pack8<T>(o));
+    }
+  }
+}
+
+cudaError_t bias_swiglu(const void* z, const void* bias, const void* dh, void* out, size_t rows, int width, int dtype, bool bwd, int num_sms,
+                        cudaStream_t st) {
+  if (width % 8) return cudaErrorInvalidValue;
+  const size_t total = rows * (size_t)(width / 8);
+  if (!total) return cudaSuccess;
+  const int threads = 256, grid = ew_grid(total, threads, num_sms);
+#define PFX_LAUNCH(T)                                                                                                              \
+  if (bwd) bias_swiglu_kernel<T, true><<<grid, threads, 0, st>>>((const T*)z, (const T*)bias, (const T*)dh, (T*)out, total, width / 8); \
+  else bias_swiglu_kernel<T, false><<<grid, threads, 0, st>>>((const T*)z, (const T*)bias, nullptr, (T*)out, total, width / 8);
   if (dtype == 1) { PFX_LAUNCH(__nv_bfloat16) } else { PFX_LAUNCH(__half) }
 #undef PFX_LAUNCH
   return cudaGetLastError();

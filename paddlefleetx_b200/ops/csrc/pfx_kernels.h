@@ -14,6 +14,9 @@ cudaError_t norm_bwd(const void* dy, const void* x, const void* w, const float* 
 
 cudaError_t bias_gelu(const void* x, const void* bias, const void* dy, void* out, size_t rows, int cols, int dtype, bool bwd, int num_sms,
                       cudaStream_t st, bool exact = false);
+// SwiGLU over pair-interleaved z [rows, 2 width] (+ bias [2 width]): fwd out = h [rows, width]; bwd (dh [rows, width]) out = dz [rows, 2 width]
+cudaError_t bias_swiglu(const void* z, const void* bias, const void* dh, void* out, size_t rows, int width, int dtype, bool bwd, int num_sms,
+                        cudaStream_t st);
 cudaError_t bias_dropout_add(const void* x, const void* bias, const void* residual, void* out, size_t rows, int cols, float p,
                              uint64_t seed, uint64_t offset, int dtype, bool bwd, int num_sms, cudaStream_t st);
 int colsum_num_parts(int rows);

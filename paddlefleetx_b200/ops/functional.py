@@ -279,17 +279,22 @@ def gemv_max_rows() -> int:
 
 
 def gemv_fused(x: torch.Tensor, weight: torch.Tensor, bias=None, ln=None, residual=None, act: Optional[str] = None) -> torch.Tensor:
-    """Decode-step linear with optional LayerNorm prologue (``ln = (gamma, beta, eps)``), GELU(tanh) and ``+ residual``:
-    ``act((LN(x)) W^T + b) + residual`` for <= 8 rows in one weight-streaming kernel (csrc/gemv_skinny.cu)."""
+    """Decode-step linear with optional LayerNorm prologue (``ln = (gamma, beta, eps)``), GELU(tanh) or SwiGLU and ``+ residual``:
+    ``act((LN(x)) W^T + b) + residual`` for <= 8 rows in one weight-streaming kernel (csrc/gemv_skinny.cu).  ``act="swiglu"`` takes
+    pair-interleaved weight rows (gate, up) and returns half as many columns (see ``bias_swiglu``)."""
+    if act not in (None, "gelu", "swiglu"):
+        raise ValueError(f"gemv_fused: act must be None, 'gelu' or 'swiglu', got {act!r}")
     if x.is_cuda and _native.available():
         _count()
         lw, lb, eps = (ln[0], ln[1], float(ln[2])) if ln is not None else (None, None, 1e-5)
         return _native.require().gemv_fused(x.contiguous(), weight, bias, lw, lb, eps, None if residual is None else residual.contiguous(),
-                                            1 if act == "gelu" else 0)
+                                            {None: 0, "gelu": 1, "swiglu": 2}[act])
     h = x if ln is None else F.layer_norm(x.float(), (x.shape[-1],), ln[0].float(), ln[1].float(), ln[2]).to(x.dtype)
     y = F.linear(h, weight, bias)
     if act == "gelu":
         y = F.gelu(y, approximate="tanh")
+    elif act == "swiglu":
+        y = _swiglu_reference(y)
     return y if residual is None else y + residual
 
 
@@ -361,6 +366,43 @@ def bias_gelu(x: torch.Tensor, bias: Optional[torch.Tensor] = None, exact: bool 
             bias = bias.to(x.dtype)
         return _BiasGeluFn.apply(x, bias, exact)
     return F.gelu(x if bias is None else x + bias, approximate="none" if exact else "tanh")
+
+
+# =============================================================================== bias + SwiGLU
+class _BiasSwigluFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, z, bias):
+        lib = _native.require()
+        z = z.contiguous()
+        ctx.save_for_backward(z, bias)
+        _count()
+        return lib.bias_swiglu_fwd(z, bias)
+
+    @staticmethod
+    def backward(ctx, gh):
+        lib = _native.require()
+        z, bias = ctx.saved_tensors
+        gz = lib.bias_swiglu_bwd(gh.contiguous(), z, bias)
+        _count()
+        gb = None
+        if bias is not None and ctx.needs_input_grad[1]:
+            gb = lib.colsum(gz.view(-1, gz.shape[-1]), False)
+            _count(2)
+        return gz, gb
+
+
+def _swiglu_reference(z: torch.Tensor) -> torch.Tensor:
+    return F.silu(z[..., 0::2]) * z[..., 1::2]
+
+
+def bias_swiglu(z: torch.Tensor, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """SwiGLU of the pair-interleaved FFN1 output ``z + bias`` ``[.., 2F]`` -> ``[.., F]``: column 2i is gate channel i, column 2i + 1 its up
+    channel, h_i = silu(gate_i) * up_i.  The kernel needs F % 8 == 0; other widths, CPU and fp32 run the torch expression."""
+    if _native_ok(z) and z.shape[-1] % 16 == 0:
+        if bias is not None and bias.dtype != z.dtype:        # O1 autocast: fp32 parameters next to bf16 activations
+            bias = bias.to(z.dtype)
+        return _BiasSwigluFn.apply(z, bias)
+    return _swiglu_reference(z if bias is None else z + bias)
 
 
 # =============================================================================== bias + dropout + residual

@@ -36,6 +36,24 @@ def check_kv_heads(m, d, compress) -> None:
                          "set Compress.Prune.prune_heads=False to prune the FFN only")
 
 
+def check_ffn_activation(m, d, compress) -> None:
+    """``Model.ffn_activation``: ``gelu`` (default) or ``swiglu`` (gated FFN of width ``ffn_hidden_size``, ``linear1`` holding gate / up pairs)."""
+    act = m.get("ffn_activation")
+    if act is None or act == "gelu":
+        return
+    if act != "swiglu":
+        raise ValueError(f"Model.ffn_activation must be gelu or swiglu, got {act!r}")
+    if (m.get("moe_configs") or {}).get("expert_mode", False):
+        raise ValueError("ffn_activation: swiglu is not supported with moe_configs (the MoE experts keep the GELU FFN)")
+    prune = compress.get("Prune") or {}
+    if prune.get("enable", False):
+        raise ValueError("Compress.Prune does not support ffn_activation: swiglu (FFN channel pruning would have to remove gate / up pairs)")
+    f, mp = m.get("ffn_hidden_size"), d.get("mp_degree", 1)
+    if f and mp > 1 and f % mp:
+        raise ValueError(f"ffn_hidden_size ({f}) must be divisible by mp_degree ({mp}) under ffn_activation: swiglu: "
+                         "tensor parallelism shards whole gate / up pairs")
+
+
 def check_config(cfg):
     g, d = cfg.Global, cfg.get("Distributed", {})
     for key in ("local_batch_size", "micro_batch_size"):
@@ -54,5 +72,6 @@ def check_config(cfg):
     if m.get("num_attention_heads") and d.get("mp_degree", 1) > 1 and m.num_attention_heads % d.mp_degree:
         raise ValueError("num_attention_heads must be divisible by mp_degree")
     check_kv_heads(m, d, cfg.get("Compress", {}) or {})
+    check_ffn_activation(m, d, cfg.get("Compress", {}) or {})
     logger.debug("config checks passed")
     return True

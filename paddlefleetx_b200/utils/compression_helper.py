@@ -179,6 +179,8 @@ def prune_model(model: nn.Module, cfg: dict) -> nn.Module:
     n_layers = 0
     for mod in model.modules():
         if hasattr(mod, "linear1") and hasattr(mod, "linear2") and hasattr(mod.linear1, "weight"):
+            if getattr(mod, "ffn_activation", "gelu") == "swiglu":
+                raise ValueError("structured pruning does not support ffn_activation: swiglu (linear1 holds gate / up pairs)")
             w1, w2 = mod.linear1.weight, mod.linear2.weight
             keep = max(int(round(w1.shape[0] * (1 - ratio) / 8)) * 8, 8)
             idx = torch.topk(_norm(w1.data, crit, 1), keep).indices.sort().values

@@ -68,6 +68,7 @@ class ModelShape:
     seq: int
     moe_experts: int = 0                 # experts per MoE layer on one rank (0 = dense)
     kv_heads: int = 0                    # K/V heads (grouped-query attention); 0 = heads
+    ffn_activation: str = "gelu"         # gelu | swiglu (FFN1 then has 2 ffn output rows: gate / up pairs)
 
     @property
     def n_kv_heads(self) -> int:
@@ -79,9 +80,15 @@ class ModelShape:
         return (self.heads + 2 * self.n_kv_heads) * (self.hidden / self.heads)
 
     @property
+    def ffn1_width(self) -> int:
+        """Output width of FFN1: f, or 2 f under SwiGLU."""
+        return 2 * self.ffn if self.ffn_activation == "swiglu" else self.ffn
+
+    @property
     def params_per_layer(self) -> float:
-        # QKV h (H + 2 Hkv) d, out-proj h^2, FFN 2 h f; biases (H + 2 Hkv) d + h + h + f, two norms 4 h
-        return self.hidden * self.qkv_width + self.hidden * self.hidden + 2 * self.hidden * self.ffn + self.qkv_width + 6 * self.hidden + self.ffn
+        # QKV h (H + 2 Hkv) d, out-proj h^2, FFN h (f1 + f) with f1 = ffn1_width; biases (H + 2 Hkv) d + h + h + f1, two norms 4 h
+        return (self.hidden * self.qkv_width + self.hidden * self.hidden + self.hidden * (self.ffn1_width + self.ffn) + self.qkv_width + 6 * self.hidden
+                + self.ffn1_width)
 
     @property
     def params(self) -> float:
@@ -98,7 +105,7 @@ class ModelShape:
             pass
         return ModelShape(layers=int(m.get("num_layers", m.get("num_hidden_layers", 12))), hidden=h, heads=int(m.get("num_attention_heads", 12)),
                           vocab=int(m.get("vocab_size", 50304)), ffn=int(m.get("ffn_hidden_size", 4 * h) or 4 * h), seq=seq,
-                          kv_heads=int(m.get("num_key_value_heads") or 0))
+                          kv_heads=int(m.get("num_key_value_heads") or 0), ffn_activation=str(m.get("ffn_activation") or "gelu"))
 
 
 @dataclass
@@ -148,7 +155,7 @@ def _layer_time(hw: Hardware, s: ModelShape, tokens: float, mp: int, sp: bool, r
     """Forward + backward of one transformer layer for ``tokens`` tokens on one GPU of an ``mp``-way tensor-parallel group."""
     h, f = s.hidden, s.ffn
     fwd_gemm = (_gemm_time(hw, tokens, s.qkv_width / mp, h) + _gemm_time(hw, tokens, h, h / mp)
-                + _gemm_time(hw, tokens, f / mp, h) + _gemm_time(hw, tokens, h, f / mp))
+                + _gemm_time(hw, tokens, s.ffn1_width / mp, h) + _gemm_time(hw, tokens, h, f / mp))
     gemm = 3.0 * fwd_gemm                                        # dgrad + wgrad have the forward's shapes
     attn_flops = 2.0 * 2.0 * tokens * s.seq * h / mp / 2.0       # causal: half of QK^T and PV
     attn_fwd, attn_bwd = attn_flops / hw.attn_fwd_flops, 2.5 * attn_flops / hw.attn_bwd_flops

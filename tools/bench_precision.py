@@ -1,7 +1,7 @@
 """float16 against bfloat16 on the headline GPT-1.3B single-GPU step, and the kernels behind it, on one H100.
 
     python tools/bench_precision.py --steps 20 --warmup 5            # arms fp16, bf16, fp16, bf16: one subprocess each
-    python tools/bench_precision.py --kernels                         # GEMM and flash-attention timings in both dtypes
+    python tools/bench_precision.py --kernels                         # GEMM, flash-attention and SwiGLU timings in both dtypes
 
 Step mode builds the exact configuration of ``bench.py --gpus 1`` (``bench.build_config``) and changes only
 ``Engine.mix_precision.dtype``.  Each arm runs in its own process under bench.py's rules: W untimed warm-up steps, then K steps
@@ -13,7 +13,10 @@ Kernel mode times the persistent GEMM at GPT-1.3B's Linear shapes (8 x 1024 toke
 the tied LM head with vocabulary 50304) in the forward and dgrad forms and in three wgrad forms: ``wgrad_bf16`` stores into a 16-bit
 [out, in] gradient buffer (out mode 0, what a training step without fp32 main gradients runs on a fresh gradient), ``wgrad_f32`` stores
 into an fp32 main gradient (out mode 1) and ``wgrad_f32acc`` accumulates into it (out mode 2).  Each row gives TFLOP/s and the share of
-the H100 SXM data-sheet dense rate (989 TFLOP/s).  Flash attention forward + backward runs at b 8, s 1024, h 16, d 128 (causal).  Both dtypes.
+the H100 SXM data-sheet dense rate (989 TFLOP/s).  Flash attention forward + backward runs at b 8, s 1024, h 16, d 128 (causal).  The
+SwiGLU kernels run at the shapes of the SwiGLU GPT-1.3B recipe (F = 5632): ``bias_swiglu`` forward and backward over 8 x 1024 tokens, and
+the LayerNorm + FFN1 + SwiGLU decode GEMV for 1 and 8 rows.  They are bandwidth-bound, so their rows give the bytes the kernel must move
+over its time and the share of the data-sheet HBM3 bandwidth (3.35 TB/s).  Both dtypes.
 """
 from __future__ import annotations
 
@@ -158,6 +161,31 @@ def run_kernels() -> list:
                          tflops=round(flops / ms_f / 1e9, 1), **info))
         rows.append(dict(kernel="attention_bwd_b8_s1024_h16_d128_causal", dtype=str(dt).split(".")[-1], ms=round(ms_b, 4),
                          tflops=round(2.5 * flops / ms_b / 1e9, 1), **info))
+        rows += _swiglu_rows(lib, dt, tokens, h, info)
+    return rows
+
+
+def _swiglu_rows(lib, dt, tokens: int, h: int, info: dict) -> list:
+    """bias_swiglu forward / backward and the SwiGLU decode GEMV at GPT-1.3B SwiGLU shapes (F = 5632), as bytes moved / time."""
+    import torch
+
+    f, e = 5632, 2                                            # F, bytes per 16-bit element
+    z = torch.randn(tokens, 2 * f, device="cuda", dtype=dt)
+    bias = torch.randn(2 * f, device="cuda", dtype=dt) * 0.1
+    dh = torch.randn(tokens, f, device="cuda", dtype=dt)
+    w = torch.randn(2 * f, h, device="cuda", dtype=dt) * 0.02
+    gamma, beta = torch.ones(h, device="cuda", dtype=dt), torch.zeros(h, device="cuda", dtype=dt)
+    cases = [("bias_swiglu_fwd_8192x5632", lambda: lib.bias_swiglu_fwd(z, bias), e * (tokens * 3 * f + 2 * f)),   # z + bias in, h out
+             ("bias_swiglu_bwd_8192x5632", lambda: lib.bias_swiglu_bwd(dh, z, bias), e * (tokens * 5 * f + 2 * f))]  # dh, z, bias in, dz out
+    for m in (1, 8):
+        x = torch.randn(m, h, device="cuda", dtype=dt)
+        cases.append((f"gemv_ln_ffn1_swiglu_rows{m}_{2 * f}x{h}", lambda x=x: lib.gemv_fused(x, w, bias, gamma, beta, 1e-5, None, 2),
+                      e * (2 * f * h + 2 * f + m * h + 2 * h + m * f)))
+    rows = []
+    for name, fn, nbytes in cases:
+        ms = _time_ms(fn)
+        rows.append(dict(kernel=name, dtype=str(dt).split(".")[-1], ms=round(ms, 4), gb_per_s=round(nbytes / ms / 1e6, 1),
+                         pct_of_3350=round(100.0 * nbytes / ms / 1e6 / 3350.0, 1), **info))
     return rows
 
 

@@ -3,6 +3,8 @@
     moe    GPT-MoE 8 x 1.3B, expert parallel over the data-parallel ranks, gshard top-2, 2 experts / rank   (tokens/s)
     vit    ViT-L/16 384^2 fine-tune, ZeRO stage 2 over all ranks, 32 images / GPU                            (images/s)
     ernie  ERNIE 10B-class encoder, mp x ZeRO stage 3                                                        (tokens/s)
+    gpt-1.3b    GPT 1.3B (tanh-GELU FFN, 4h), data parallel, 8 x 1024 tokens / GPU                          (tokens/s)
+    gpt-swiglu  the same model with the SwiGLU FFN (Model.ffn_activation: swiglu, F = 5632)                  (tokens/s)
 
 Synthetic data of the named shape, random-init weights, bf16.  Same contract as bench.py: W warm-up steps, K steps timed with CUDA
 events between barriers, max over ranks, nvidia-smi clocks / throttle reasons sampled during the timed region, the exposed-
@@ -27,7 +29,7 @@ CFG = os.path.join(ROOT, "paddlefleetx_b200", "configs")
 
 def parse():
     p = argparse.ArgumentParser()
-    p.add_argument("--workload", required=True, choices=["moe", "vit", "ernie"])
+    p.add_argument("--workload", required=True, choices=["moe", "vit", "ernie", "gpt-1.3b", "gpt-swiglu"])
     p.add_argument("--gpus", type=int, default=1)
     p.add_argument("--steps", type=int, default=5)
     p.add_argument("--warmup", type=int, default=3)
@@ -57,7 +59,30 @@ def main():
     dev = torch.device("cuda", torch.cuda.current_device())
     common = ["Engine.max_steps=1000000", "Engine.eval_freq=-1", "Engine.logging_freq=1000000", "Engine.save_load.save_steps=-1",
               "Engine.mix_precision.enable=True", "Engine.mix_precision.dtype=bfloat16", "Global.global_batch_size=None"]
-    if a.workload == "moe":
+    if a.workload in ("gpt-1.3b", "gpt-swiglu"):
+        local = a.local_batch or 8
+        swiglu = a.workload == "gpt-swiglu"
+        ov = common + [f"Global.local_batch_size={local}", f"Global.micro_batch_size={local}", f"Distributed.dp_degree={world}",
+                       "Distributed.mp_degree=1", "Distributed.pp_degree=1", "Distributed.sharding.sharding_degree=1"]
+        if a.layers:
+            ov.append(f"Model.num_layers={a.layers}")
+        recipe = "pretrain_gpt_1.3B_swiglu_single_card.yaml" if swiglu else "pretrain_gpt_1.3B_single_card.yaml"
+        cfg = C.get_config(os.path.join(CFG, "nlp/gpt", recipe), ov, nranks=world)
+        seq = 1024
+        cfg.Data.Train["dataset"] = C.AttrDict(name="SyntheticGPTDataset", max_seq_len=seq, vocab_size=cfg.Model.vocab_size)
+        cfg.Data.Train["loader"] = C.AttrDict(num_workers=0, collate_fn="gpt_collate_fn")
+        unit, per_step = "tokens/s", local * seq * world
+        from paddlefleetx_b200.models.language_model.gpt.model import swiglu_ffn_size
+
+        h = cfg.Model.hidden_size
+        ffn = cfg.Model.get("ffn_hidden_size") or (swiglu_ffn_size(h) if swiglu else 4 * h)
+        name = f"GPT 1.3B ({'SwiGLU' if swiglu else 'GELU'} FFN, F = {ffn}), dp{world}, {local} x {seq} tokens/GPU, recompute {cfg.Model.get('use_recompute')}"
+
+        def make_batch(g):
+            t = torch.randint(0, cfg.Model.vocab_size, (local, seq + 1), generator=g)
+            pos = torch.arange(seq).unsqueeze(0).expand(local, seq).contiguous()
+            return [t[:, :-1].contiguous(), pos, t[:, 1:].contiguous(), torch.ones(local, seq)]
+    elif a.workload == "moe":
         local = a.local_batch or 8
         ov = common + [f"Global.local_batch_size={local}", f"Global.micro_batch_size={local}", f"Distributed.dp_degree={world}",
                        "Distributed.mp_degree=1", "Distributed.pp_degree=1", "Distributed.sharding.sharding_degree=1",
