@@ -111,7 +111,7 @@ std::vector<at::Tensor> gemm_bias_gelu_dual(const at::Tensor& x, const at::Tenso
 }
 
 // FFN2 dgrad with the GELU derivative applied in the epilogue: dz = (dy W) * gelu'(z);  w is [K = out_features, N = in_features].
-at::Tensor gemm_dgelu(const at::Tensor& dy, const at::Tensor& w, const at::Tensor& z) {
+at::Tensor gemm_dgelu(const at::Tensor& dy, const at::Tensor& w, const at::Tensor& z, int64_t config) {
   TORCH_CHECK(dy.is_cuda() && dy.dim() == 2 && w.dim() == 2 && z.dim() == 2 && dy.is_contiguous() && w.is_contiguous() && z.is_contiguous(), "gemm_dgelu: contiguous 2-D");
   TORCH_CHECK(dy.size(1) == w.size(0) && z.size(0) == dy.size(0) && z.size(1) == w.size(1), "gemm_dgelu: dy [M,K], w [K,N], z [M,N]");
   TORCH_CHECK(is_16bit(dy) && w.scalar_type() == dy.scalar_type() && z.scalar_type() == dy.scalar_type(), "gemm_dgelu: bf16 or fp16 operands of one dtype");
@@ -122,7 +122,7 @@ at::Tensor gemm_dgelu(const at::Tensor& dy, const at::Tensor& w, const at::Tenso
   g.a = dy.data_ptr(); g.b = w.data_ptr(); g.d = dz.data_ptr(); g.aux = z.data_ptr(); g.ld_aux = (int)z.stride(0);
   g.M = (int)dy.size(0); g.N = (int)w.size(1); g.K = (int)dy.size(1);
   g.lda = (int)dy.stride(0); g.ldb = (int)w.stride(0); g.ldd = (int)dz.stride(0);
-  g.a_kmajor = true; g.b_kmajor = false; g.out_mode = 0; g.epilogue = pfx::EPI_DGELU; g.ab_format = dtype_code(dy); g.num_sms = num_sms(); g.config = 0;
+  g.a_kmajor = true; g.b_kmajor = false; g.out_mode = 0; g.epilogue = pfx::EPI_DGELU; g.ab_format = dtype_code(dy); g.num_sms = num_sms(); g.config = (int)config;
   PFX_CUDA_CHECK(pfx::gemm_wgmma(g, cur_stream()));
   return dz;
 }
@@ -142,7 +142,7 @@ void gemm_rs_scatter(const at::Tensor& a, const at::Tensor& b, const std::vector
   g.M = (int)M; g.N = (int)N; g.K = (int)K;
   g.lda = (int)a.stride(0); g.ldb = (int)b.stride(0); g.ldd = (int)N;
   g.a_kmajor = a_kmajor; g.b_kmajor = b_kmajor; g.out_mode = 3; g.epilogue = pfx::EPI_NONE; g.ab_format = 1;
-  g.num_sms = num_sms(); g.config = config ? (int)config : 2;
+  g.num_sms = num_sms(); g.config = (int)config;
   for (int i = 0; i < world; ++i) g.comm.peer_out[i] = reinterpret_cast<void*>((uintptr_t)peer_staging[i]);
   g.comm.rows_per_rank = (int)rows_per_rank; g.comm.my_rank = (int)my_rank; g.comm.world = world; g.comm.ag_world = 0;
   PFX_CUDA_CHECK(pfx::gemm_wgmma(g, cur_stream()));
@@ -174,7 +174,7 @@ at::Tensor gemm_ag(const at::Tensor& a_local, const at::Tensor& b, const at::Ten
   g.M = (int)M; g.N = (int)N; g.K = (int)K;
   g.lda = (int)K; g.ldb = (int)b.stride(0); g.ldd = (int)N;
   g.a_kmajor = true; g.b_kmajor = b_kmajor; g.out_mode = 0; g.epilogue = g.bias ? pfx::EPI_BIAS : pfx::EPI_NONE; g.ab_format = 1;
-  g.num_sms = num_sms(); g.config = config ? (int)config : 2;
+  g.num_sms = num_sms(); g.config = (int)config;
   for (int i = 0; i < world; ++i) {
     g.comm.peer_gather[i] = reinterpret_cast<void*>((uintptr_t)peer_gather[i]);
     g.comm.peer_flags[i] = reinterpret_cast<uint32_t*>((uintptr_t)peer_flags[i]);
@@ -1140,7 +1140,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("attention_decode", &attention_decode);
   m.def("attention_decode_packed", &attention_decode_packed);
   m.def("gemm_bias_gelu_dual", &gemm_bias_gelu_dual);
-  m.def("gemm_dgelu", &gemm_dgelu);
+  m.def("gemm_dgelu", &gemm_dgelu, py::arg("dy"), py::arg("w"), py::arg("z"), py::arg("config") = 0);
   m.def("gemv_skinny", &gemv_skinny);
   m.def("gemm_smallm", &gemm_smallm);
   m.def("gemv_w8a8", &gemv_w8a8, py::arg("xq"), py::arg("wq"), py::arg("xs"), py::arg("ws"), py::arg("bias") = py::none(),

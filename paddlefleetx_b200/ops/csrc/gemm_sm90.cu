@@ -11,6 +11,10 @@
 //     warpgroups, each wgmma m64 x BLOCK_N x 16 over its 64 rows of the 128 x BLOCK_N tile, then the epilogue from its
 //     accumulator fragment (registers -> swizzled smem -> TMA store).  One k-block of wgmma stays in flight while the next
 //     is issued; the producer runs ahead into the next tile during the epilogue.
+//   * tiles: 128 x 128 (288 threads) everywhere, and 128 x 256 (384 threads: warpgroup 2 is the producer and hands its registers to
+//     the consumers) for the plain 16-bit-output GEMM when the caller asks for it (GemmArgs::config == 1).  The wide tile fills the
+//     SM's registers and shared memory, so no side-stream kernel fits beside it: the training step asks for it in the backward only,
+//     where the single-GPU side stream carries nothing but the gradient-norm reduction (ops/functional.py).
 //
 // Fused compute+collective modes (tensor/sequence parallel linears, see parallel/fused_tp.py):
 //   * kOutMode = 3  "GEMM -> reduce-scatter": the epilogue stores each finished tile straight into the DESTINATION
@@ -35,12 +39,22 @@ constexpr int kBlockM = 128;   // rows of A per CTA: two consumer warpgroups of 
 constexpr int kBlockK = 64;    // 64 x 2 B = one 128-byte swizzle span
 constexpr int kMmaK = 16;
 constexpr int kNumConsumerWarps = 8;
-constexpr int kNumThreads = 288;   // warps 0-7 = two consumer warpgroups, warp 8 = TMA producer (ptxas allots 168 registers per thread)
 constexpr int kGroupM = 16;    // tile-raster group height (L2 reuse)
 constexpr int kStoreCols = 64; // columns per TMA-store box (128 B of bf16)
+constexpr int kWideN = 256;    // BLOCK_N of the wide tile
+// Wide tile: the launch gives 168 registers x 384 threads; the producer warpgroup drops to 40 and the consumers rise to 232
+// (232 x 256 + 40 x 128 = 168 x 384), room for a 64 x 256 fp32 accumulator (128 registers) per consumer thread.
+constexpr int kWideProducerRegs = 40;
+constexpr int kWideConsumerRegs = 232;
+static_assert(kWideConsumerRegs * 2 * 128 + kWideProducerRegs * 128 <= 168 * 384, "register reallocation exceeds the launch allocation");
 
 template <int kBlockN>
 struct GemmSmem {
+  static_assert(kBlockN == 128 || kBlockN == kWideN, "tiles are 128 x 128 or 128 x 256");
+  static constexpr bool kWide = kBlockN == kWideN;
+  // 128 x 128: warps 0-7 = two consumer warpgroups, warp 8 = TMA producer (ptxas allots 168 registers per thread).
+  // 128 x 256: warps 0-7 = consumers, warpgroup 2 (warps 8-11) = producer, one elected thread of warp 8 issues the TMA loads.
+  static constexpr int kThreads = kWide ? 384 : 288;
   static constexpr int kABytes = kBlockM * kBlockK * 2;
   static constexpr int kBBytes = kBlockN * kBlockK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
@@ -49,10 +63,13 @@ struct GemmSmem {
   static constexpr int kBarrierBytes = 1024;
   // 12 KB of the SM's 228 KB stay free: a co-resident communication / optimizer CTA needs its own 1 KB system reservation (plus any static
   // shared memory), and a GEMM that fills the SM to the last kilobyte serialises with every kernel on the side streams instead of sharing it.
-  static constexpr int kHeadroom = 12 * 1024;
+  // The wide tile takes the whole SM: it keeps no headroom.
+  static constexpr int kHeadroom = kWide ? 0 : 12 * 1024;
   static constexpr int kBudget = 227 * 1024 - kHeadroom - 1024 /*align slack*/ - kBarrierBytes - kNumEpiBufs * kEpiBytes;
   static constexpr int kStages = (kBudget / kStageBytes) > 8 ? 8 : (kBudget / kStageBytes);
   static constexpr int kTotal = 1024 + kStages * kStageBytes + kNumEpiBufs * kEpiBytes + kBarrierBytes;
+  static_assert(kTotal <= 227 * 1024, "shared memory exceeds the 227 KB a CTA may use");
+  static_assert(!kWide || kStages == 4, "the wide tile runs four 48 KB stages");
 };
 
 struct TileCoord { int m_blk, n_blk; };
@@ -67,6 +84,13 @@ __device__ __forceinline__ TileCoord tile_coord(int tile, int num_m_blocks, int 
   int m = first_m + in_group % group_m;
   if (m_rotate) { m += m_rotate; if (m >= num_m_blocks) m -= num_m_blocks; }
   return {m, in_group / group_m};
+}
+
+// A copy of x the compiler cannot see through: what is computed from it is computed where the copy is made, not hoisted or shared.
+template <typename T>
+__device__ __forceinline__ T opaque(T x) {
+  asm volatile("" : "+r"(x));
+  return x;
 }
 
 __device__ __forceinline__ uint32_t ld_acquire_sys(const uint32_t* p) {
@@ -114,7 +138,7 @@ __device__ void ag_push_role(const GemmComm& c, int comm_cta, int num_comm_ctas,
 // kOutMode: 0 = bf16/fp16 via TMA store, 1 = fp32 direct store, 2 = fp32 direct accumulate (D += acc),
 //           3 = bf16 scatter into the destination rank's staging buffer over NVLink (GEMM -> reduce-scatter)
 template <int kBlockN, bool kAK, bool kBK, int kOutMode, bool kBf16>
-__global__ void __launch_bounds__(kNumThreads, 1)
+__global__ void __launch_bounds__(GemmSmem<kBlockN>::kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_a_local,
                   float* __restrict__ out_f32, const uint16_t* __restrict__ bias,
@@ -124,6 +148,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   using S = GemmSmem<kBlockN>;
   constexpr int kStages = S::kStages;
   static_assert(kStages >= 2, "pipeline needs at least two stages");
+  static_assert(!S::kWide || kOutMode == 0, "the wide tile serves the 16-bit TMA-store output only");
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -136,11 +161,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   const uint32_t warp = warp_id();
   const uint32_t lane = lane_id();
 
-  const int num_m_blocks = (M + kBlockM - 1) / kBlockM;
-  const int num_n_blocks = (N + kBlockN - 1) / kBlockN;
-  const int num_tiles = num_m_blocks * num_n_blocks;
-  const int num_k_blocks = (K + kBlockK - 1) / kBlockK;
-  const int num_comm_ctas = comm.ag_world > 1 ? comm.num_comm_ctas : 0;
+  int num_m_blocks, num_n_blocks, num_tiles, num_k_blocks;
+  auto tile_grid = [&](int m, int n, int k) {
+    num_m_blocks = (m + kBlockM - 1) / kBlockM;
+    num_n_blocks = (n + kBlockN - 1) / kBlockN;
+    num_tiles = num_m_blocks * num_n_blocks;
+    num_k_blocks = (k + kBlockK - 1) / kBlockK;
+  };
+  tile_grid(M, N, K);
+  // The wide tile never runs a collective mode (the host routes those to 128 x 128).
+  const int num_comm_ctas = !S::kWide && comm.ag_world > 1 ? comm.num_comm_ctas : 0;
   const int num_ctas = (int)gridDim.x - num_comm_ctas;
   const int cta_id = blockIdx.x;
   if (cta_id >= num_ctas) {   // ---- communication CTAs (all-gather -> GEMM mode): no barriers
@@ -148,7 +178,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     return;
   }
   int m_rotate = 0;
-  if (comm.rows_per_rank > 0 && comm.world > 1) {   // start one rank "after" ourselves: remote tiles first (RS) /
+  if (!S::kWide && comm.rows_per_rank > 0 && comm.world > 1) {   // start one rank "after" ourselves: remote tiles first (RS) /
     const int blocks_per_rank = comm.rows_per_rank / kBlockM;                 // local tiles first (AG)
     m_rotate = ((comm.my_rank + (kOutMode == 3 ? 1 : 0)) % comm.world) * blocks_per_rank;
   }
@@ -163,8 +193,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   }
   __syncthreads();
 
-  if (warp == 8) {
+  if (warp >= kNumConsumerWarps) {
     // ===================================================================== TMA producer
+    if constexpr (S::kWide) {
+      setmaxnreg_dec<kWideProducerRegs>();
+      // ptxas spills what is live across setmaxnreg, so the warp test and the tile grid are formed anew here
+      if ((threadIdx.x >> 5) != kNumConsumerWarps) return;   // warps 9-11 of the producer warpgroup have no work
+      tile_grid(opaque(M), opaque(N), opaque(K));
+    }
     if (elect_one()) {
       int stage = 0; uint32_t phase = 0;
       for (int tile = cta_id; tile < num_tiles; tile += num_ctas) {
@@ -224,6 +260,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     }
   } else {
     // ===================================================================== consumers: mainloop (wgmma) + epilogue, 64 rows per warpgroup
+    if constexpr (S::kWide) {
+      setmaxnreg_inc<kWideConsumerRegs>();
+      tile_grid(opaque(M), opaque(N), opaque(K));
+    }
     const uint32_t wg = warp >> 2;
     const uint32_t row_lo = wg * 64u + (warp & 3u) * 16u + (lane >> 2);   // this thread's rows inside the CTA tile: row_lo and row_lo + 8
     const uint32_t col_in8 = (lane & 3u) * 2u;                            // ... and its column pair inside every 8-column group
@@ -278,9 +318,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       for (int c = 0; c < kBlockN / kStoreCols; ++c) {
         const int col0 = col_tile + c * kStoreCols;
         const int cb = col0 + (int)col_in8;       // column of v[4 j] / v[4 j + 2]; v[4 j + 1] / v[4 j + 3] are one to the right
-        float v[32];                              // v[4 j + e]: row row_lo + 8 (e / 2), column cb + 8 j + (e % 2)
+        // v[4 j + e]: row row_lo + 8 (e / 2), column cb + 8 j + (e % 2).  The wide tile has no registers for a copy of the chunk next to
+        // its 128 accumulators and works on them in place (it never runs grouped, so its k-range is never empty).
+        float v_copy[S::kWide ? 1 : 32];
+        float* v = acc + c * 32;
+        if constexpr (!S::kWide) {
+          v = v_copy;
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = empty_k ? 0.f : acc[c * 32 + i];
+          for (int i = 0; i < 32; ++i) v[i] = empty_k ? 0.f : acc[c * 32 + i];
+        }
         if (epilogue == EPI_BIAS || epilogue == EPI_BIAS_GELU || epilogue == EPI_BIAS_GELU_DUAL) {
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
@@ -290,7 +336,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             }
           }
         }
-        if (epilogue == EPI_BIAS_GELU || epilogue == EPI_GELU) {
+        if (!S::kWide && (epilogue == EPI_BIAS_GELU || epilogue == EPI_GELU)) {   // the wide tile serves EPI_NONE / EPI_BIAS / EPI_DGELU
 #pragma unroll
           for (int i = 0; i < 32; ++i) v[i] = gelu_tanh(v[i]);
         }
@@ -321,11 +367,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 #pragma unroll
           for (int hh = 0; hh < 2; ++hh) {
             const uint32_t r = row_lo + 8u * hh;
-            const uint32_t sbase = smem_epi + buf * S::kEpiBytes + r * 128u + col_in8 * 2u;
+            uint32_t sbase = smem_epi + buf * S::kEpiBytes + r * 128u + col_in8 * 2u;
+            uint32_t r_sw = r & 7u;
+            // Wide tile: the compiler would keep the 16 swizzled store addresses live across the tile loop, and beside 128 accumulators
+            // they spill.  Opaque copies make it form them anew for each chunk (a few integer ops).
+            if constexpr (S::kWide) { sbase = opaque(sbase); r_sw = opaque(r_sw); }
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
               const uint32_t p = pack_16x2<kBf16>(v[4 * j + 2 * hh], v[4 * j + 2 * hh + 1]);
-              asm volatile("st.shared.b32 [%0], %1;" ::"r"(sbase + (((uint32_t)j ^ (r & 7u)) << 4)), "r"(p) : "memory");
+              asm volatile("st.shared.b32 [%0], %1;" ::"r"(sbase + (((uint32_t)j ^ r_sw) << 4)), "r"(p) : "memory");
             }
           }
           fence_proxy_async_smem();
@@ -346,7 +396,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           ++store_iter;
           };
           store_chunk(&tmap_d);
-          if (epilogue == EPI_BIAS_GELU_DUAL) {
+          if (!S::kWide && epilogue == EPI_BIAS_GELU_DUAL) {
 #pragma unroll
             for (int i = 0; i < 32; ++i) v[i] = gelu_tanh(v[i]);
             store_chunk(&tmap_d2);
@@ -566,7 +616,7 @@ static cudaError_t launch_cfg(const GemmArgs& g, cudaStream_t stream) {
 
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(ctas);
-  cfg.blockDim = dim3(kNumThreads);
+  cfg.blockDim = dim3(S::kThreads);
   cfg.dynamicSmemBytes = S::kTotal;
   cfg.stream = stream;
   const cudaError_t le = cudaLaunchKernelEx(&cfg, kern, ta, tb, td, tal, reinterpret_cast<float*>(g.d), reinterpret_cast<const uint16_t*>(g.bias),
@@ -599,6 +649,11 @@ static cudaError_t launch_out(const GemmArgs& g, cudaStream_t s) {
 
 cudaError_t gemm_wgmma(const GemmArgs& g, cudaStream_t stream) {
   if (g.M <= 0 || g.N <= 0 || g.K <= 0) return cudaSuccess;
+  // The wide tile is compiled for the plain GEMM with a 16-bit output and the epilogues of the backward pass; any other request runs
+  // 128 x 128 and gives the same result.
+  const bool wide = g.config == 1 && g.out_mode == 0 && g.group.mode == 0 && g.comm.rows_per_rank == 0 && g.comm.ag_world <= 1 &&
+                    (g.epilogue == EPI_NONE || g.epilogue == EPI_BIAS || g.epilogue == EPI_DGELU);
+  if (wide) return launch_major<kWideN, 0>(g, stream);
   return launch_out<128>(g, stream);   // 128 x 128 tiles: 64 accumulator registers per consumer thread (162-168 registers in all; the eight out-mode-1 variants spill 44 bytes)
 }
 

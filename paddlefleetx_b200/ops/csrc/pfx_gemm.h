@@ -57,7 +57,7 @@ struct GemmArgs {
   int epilogue;      // Epilogue
   int ab_format;     // 0 = fp16, 1 = bf16
   int num_sms;
-  int config;        // 0 = auto
+  int config;        // 1 = 128 x 256 tile requested (honoured for out mode 0 with EPI_NONE / EPI_BIAS / EPI_DGELU, else 128 x 128); 0 = 128 x 128
   GemmComm comm;     // zero-initialised = plain GEMM
   GemmGroup group;   // mode 0 = plain GEMM
 };

@@ -35,6 +35,13 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
+// Register reallocation between the warpgroups of a CTA: every thread of the warpgroup executes the same instruction; the count is a
+// multiple of 8 in [24, 256].
+template <int kRegs>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+template <int kRegs>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+
 // ------------------------------------------------------------------ cluster
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;

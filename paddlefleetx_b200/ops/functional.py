@@ -61,6 +61,22 @@ def _gemm_ok(x: torch.Tensor, *dims: int) -> bool:
 # =============================================================================== linear
 EPI_NONE, EPI_BIAS, EPI_BIAS_GELU, EPI_GELU = 0, 1, 2, 3
 
+# The GEMM's ``config`` argument: 1 asks for the 128 x 256 tile (csrc/gemm_sm90.cu), 0 for 128 x 128.  The wide tile takes all of an SM's
+# registers and shared memory, so no side-stream kernel runs beside it.  The forward keeps 128 x 128 because the overlapped AdamW update
+# of the previous step runs beneath it; the backward asks for the wide tile, since on one GPU the side stream then carries only the
+# gradient-norm reduction.  ``FusedAdamW`` turns this off when it overlaps gradient collectives with the backward (more than one replica).
+_wide_backward = 1
+
+
+def set_wide_backward(on: bool) -> None:
+    """Let the backward GEMMs run 128 x 256 tiles (on by default)."""
+    global _wide_backward
+    _wide_backward = 1 if on else 0
+
+
+def wide_backward() -> bool:
+    return _wide_backward == 1
+
 
 def _wgrad(lib, g2: torch.Tensor, x2: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
     """dW = g2^T x2.  With a flat gradient buffer behind the weight (``weight.main_grad``, set up by FusedAdamW) the GEMM stores or
@@ -71,16 +87,16 @@ def _wgrad(lib, g2: torch.Tensor, x2: torch.Tensor, weight: torch.Tensor) -> tor
         if main_grad.dtype == torch.float32:
             lib.gemm(g2, x2, None, main_grad, False, False, EPI_NONE, 1 if fresh else 2, 0)   # main_grad (+)= dY^T X
         elif fresh:
-            lib.gemm(g2, x2, None, main_grad, False, False, EPI_NONE, 0, 0)
+            lib.gemm(g2, x2, None, main_grad, False, False, EPI_NONE, 0, _wide_backward)
         else:
-            main_grad.add_(lib.gemm(g2, x2, None, None, False, False, EPI_NONE, 0, 0))
+            main_grad.add_(lib.gemm(g2, x2, None, None, False, False, EPI_NONE, 0, _wide_backward))
         weight._grad_fresh = False
         # autograd still needs a tensor so that post-accumulate hooks (DP / ZeRO bucket readiness) fire; the optimizer's hook
         # drops ``weight.grad`` when this flag is set.
         weight.grad_added_to_main_grad = True
         gw = torch.empty_like(weight)
     else:
-        gw = lib.gemm(g2, x2, None, None, False, False, EPI_NONE, 0, 0)
+        gw = lib.gemm(g2, x2, None, None, False, False, EPI_NONE, 0, _wide_backward)
     _count()
     return gw
 
@@ -112,7 +128,7 @@ class _FusedFFNFn(torch.autograd.Function):
         g2 = gy.reshape(-1, gy.shape[-1])
         if not g2.is_contiguous():
             g2 = g2.contiguous()
-        dz = lib.gemm_dgelu(g2, w2, z)                      # (dy W2) * gelu'(z)
+        dz = lib.gemm_dgelu(g2, w2, z, _wide_backward)      # (dy W2) * gelu'(z)
         _count()
         gw2 = _wgrad(lib, g2, g, w2) if ctx.needs_input_grad[3] else None
         gb1 = None
@@ -122,7 +138,7 @@ class _FusedFFNFn(torch.autograd.Function):
         gw1 = _wgrad(lib, dz, x2, w1) if ctx.needs_input_grad[1] else None
         gx = None
         if ctx.needs_input_grad[0]:
-            gx = lib.gemm(dz, w1, None, None, True, False, EPI_NONE, 0, 0).view(ctx.x_shape)
+            gx = lib.gemm(dz, w1, None, None, True, False, EPI_NONE, 0, _wide_backward).view(ctx.x_shape)
             _count()
         gb2 = None
         if ctx.has_b2 and ctx.needs_input_grad[4]:
@@ -170,7 +186,7 @@ class _LinearFn(torch.autograd.Function):
             g2 = g2.contiguous()
         gx = gw = gb = None
         if ctx.needs_input_grad[0]:
-            gx = lib.gemm(g2, weight, None, None, True, False, EPI_NONE, 0, 0).view(ctx.x_shape)
+            gx = lib.gemm(g2, weight, None, None, True, False, EPI_NONE, 0, _wide_backward).view(ctx.x_shape)
             _count()
         if ctx.needs_input_grad[1]:
             gw = _wgrad(lib, g2, x2, weight)

@@ -113,6 +113,9 @@ class FusedAdamW:
         self.sh_rank = C.group_rank(self.sh_group)
         self.dp_world = C.group_size(self.dp_group)
         self.replicas = self.sh_world * self.dp_world          # data replicas the gradient is averaged over
+        if self.replicas > 1:
+            # gradient collectives run beside the backward GEMMs: those keep the 128 x 128 tile, which leaves room on the SM for them
+            OF.set_wide_backward(False)
         if params_are_shards:
             # ZeRO-3: the "parameters" handed in are already per-rank shards (parallel/sharding.py): no further
             # partitioning or reduce-scatter here, only the dp all-reduce, the cross-group norm and the update

@@ -13,7 +13,9 @@ Kernel mode times the persistent GEMM at GPT-1.3B's Linear shapes (8 x 1024 toke
 the tied LM head with vocabulary 50304) in the forward and dgrad forms and in three wgrad forms: ``wgrad_bf16`` stores into a 16-bit
 [out, in] gradient buffer (out mode 0, what a training step without fp32 main gradients runs on a fresh gradient), ``wgrad_f32`` stores
 into an fp32 main gradient (out mode 1) and ``wgrad_f32acc`` accumulates into it (out mode 2).  Each row gives TFLOP/s and the share of
-the H100 SXM data-sheet dense rate (989 TFLOP/s).  Flash attention forward + backward runs at b 8, s 1024, h 16, d 128 (causal).  The
+the H100 SXM data-sheet dense rate (989 TFLOP/s).  The backward forms a training step runs (every dgrad, the FFN2 dgrad with the GELU
+derivative in its epilogue, ``dgelu``, and the 16-bit wgrad) are timed at both tiles of the GEMM, ``tile`` 128x128 (config 0) and
+128x256 (config 1, what the backward asks for), alternating, two windows each; ``ms`` is their mean.  Flash attention forward + backward runs at b 8, s 1024, h 16, d 128 (causal).  The
 SwiGLU kernels run at the shapes of the SwiGLU GPT-1.3B recipe (F = 5632): ``bias_swiglu`` forward and backward over 8 x 1024 tokens, and
 the LayerNorm + FFN1 + SwiGLU decode GEMV for 1 and 8 rows.  They are bandwidth-bound, so their rows give the bytes the kernel must move
 over its time and the share of the data-sheet HBM3 bandwidth (3.35 TB/s).  Both dtypes.
@@ -118,7 +120,13 @@ def _time_ms(fn, warmup=5, window_ms=500.0) -> float:
     return e0.elapsed_time(e1) / iters
 
 
+WIDE_FORMS = ("dgrad", "dgelu", "wgrad_bf16")   # the backward forms: timed at config 0 (128 x 128) and config 1 (128 x 256)
+TILES = {0: "128x128", 1: "128x256"}
+
+
 def run_kernels() -> list:
+    """One JSON-ready row per kernel and dtype: the GEMM forms at GPT-1.3B's Linear shapes (the backward forms at both tiles), flash
+    attention forward and backward, and the SwiGLU kernels, each with the GPU name and power limit."""
     import torch
 
     from paddlefleetx_b200.ops import _native
@@ -136,17 +144,28 @@ def run_kernels() -> list:
             dy = torch.randn(tokens, n_out, device="cuda", dtype=dt)
             main_grad = torch.zeros(n_out, n_in, device="cuda")
             grad = torch.empty(n_out, n_in, device="cuda", dtype=dt)
-            forms = {"fwd": lambda: lib.gemm(x, w, None, None, True, True, 0, 0, 0),                    # y = x W^T
-                     "dgrad": lambda: lib.gemm(dy, w, None, None, True, False, 0, 0, 0),                # dx = dy W
-                     "wgrad_bf16": lambda: lib.gemm(dy, x, None, grad, False, False, 0, 0, 0),          # grad = dy^T x (16-bit)
-                     "wgrad_f32": lambda: lib.gemm(dy, x, None, main_grad, False, False, 0, 1, 0),      # main_grad = dy^T x
-                     "wgrad_f32acc": lambda: lib.gemm(dy, x, None, main_grad, False, False, 0, 2, 0)}   # main_grad += dy^T x
+            forms = {"fwd": lambda c: lib.gemm(x, w, None, None, True, True, 0, 0, c),                    # y = x W^T
+                     "dgrad": lambda c: lib.gemm(dy, w, None, None, True, False, 0, 0, c),                # dx = dy W
+                     "wgrad_bf16": lambda c: lib.gemm(dy, x, None, grad, False, False, 0, 0, c),          # grad = dy^T x (16-bit)
+                     "wgrad_f32": lambda c: lib.gemm(dy, x, None, main_grad, False, False, 0, 1, c),      # main_grad = dy^T x
+                     "wgrad_f32acc": lambda c: lib.gemm(dy, x, None, main_grad, False, False, 0, 2, c)}   # main_grad += dy^T x
+            z = None
+            if name == "ffn2":            # what the fused FFN's backward runs in place of the plain FFN2 dgrad: dz = (dy W2) * gelu'(z)
+                z = torch.randn(tokens, n_in, device="cuda", dtype=dt)
+                forms["dgelu"] = lambda c: lib.gemm_dgelu(dy, w, z, c)
             for form, fn in forms.items():
-                ms = _time_ms(fn)
-                tflops = 2.0 * tokens * n_out * n_in / ms / 1e9
-                rows.append(dict(kernel=f"gemm_{name}_{form}", dtype=str(dt).split(".")[-1], ms=round(ms, 4), tflops=round(tflops, 1),
-                                 pct_of_989=round(100.0 * tflops / 989.0, 1), **info))
-            del x, w, dy, main_grad, grad
+                configs = (0, 1) if form in WIDE_FORMS else (0,)
+                times = {c: [] for c in configs}
+                for _ in range(2 if len(configs) > 1 else 1):
+                    for c in configs:
+                        times[c].append(_time_ms(lambda: fn(c)))
+                for c in configs:
+                    ms = sum(times[c]) / len(times[c])
+                    tflops = 2.0 * tokens * n_out * n_in / ms / 1e9
+                    rows.append(dict(kernel=f"gemm_{name}_{form}", tile=TILES[c], dtype=str(dt).split(".")[-1], ms=round(ms, 4),
+                                     ms_windows=[round(t, 4) for t in times[c]], tflops=round(tflops, 1),
+                                     pct_of_989=round(100.0 * tflops / 989.0, 1), **info))
+            del x, w, dy, main_grad, grad, z
         b, s, nh, d = 8, 1024, 16, 128
         mix = torch.randn(b, s, nh, 3, d, device="cuda", dtype=dt)
         q, k, v = mix.unbind(3)
