@@ -9,7 +9,10 @@ pre-processed corpora and caches are reusable.  Differences:
     downloads the vocab): ``eos_id`` defaults to 50256 and is configurable,
   * EOS loss-masking is an explicit switch ``mask_eos`` (default False = the reference's *actual* behaviour:
     its mask expression compares a python list with an int and masks nothing — SURVEY F8),
-  * ``SyntheticGPTDataset`` produces uniform random tokens of the same 4-tuple shape for benchmarking.
+  * ``SyntheticGPTDataset`` produces uniform random tokens of the same 4-tuple shape for benchmarking,
+  * ``reset_position_ids`` restarts the position ids at 0 at each document start inside a sample (Megatron's switch of that name; the
+    boundaries come from the sample's own document pieces, not from EOS tokens), so that ``Model.reset_attention_mask`` keeps attention
+    inside each document.  A sample that starts in the middle of a document counts its first piece from 0.
 """
 from __future__ import annotations
 
@@ -135,6 +138,14 @@ def _shuffle_order(n_first: int, total: int, rng: np.random.RandomState) -> np.n
     return np.concatenate([first, last])
 
 
+def document_positions(piece_lengths: Sequence[int], n: int) -> np.ndarray:
+    """Position ids of the first ``n`` tokens of a sample made of consecutive document pieces of the given lengths: 0, 1, ... restarting
+    at every piece."""
+    lens = np.asarray(piece_lengths, dtype=np.int64)
+    starts = np.concatenate([[0], np.cumsum(lens)[:-1]])
+    return (np.arange(int(lens.sum()), dtype=np.int64) - np.repeat(starts, lens))[:n]
+
+
 def python_sample_idx(sizes: np.ndarray, doc_idx: np.ndarray, seq_len: int, num_epochs: int, tokens_per_epoch: int) -> np.ndarray:
     """Pure-python twin of the C++ ``build_sample_idx`` (used as its test oracle and as a fallback)."""
     n = (num_epochs * tokens_per_epoch - 1) // seq_len
@@ -203,7 +214,7 @@ def construct_samples_and_shuffle_data(name, data_prefix, documents, sizes, num_
 
 class GPTDataset(torch.utils.data.Dataset):
     def __init__(self, input_dir: str, split: Sequence[float], max_seq_len: int, num_samples: int, mode: str, model_type: str = "GPT",
-                 seed: int = 1234, eos_id: int = 50256, mask_eos: bool = False, **unused):
+                 seed: int = 1234, eos_id: int = 50256, mask_eos: bool = False, reset_position_ids: bool = False, **unused):
         if mode not in MODE_TO_SPLIT:
             raise ValueError("valid str value for 'mode'")
         prefix = find_corpus_prefix(input_dir)
@@ -212,6 +223,7 @@ class GPTDataset(torch.utils.data.Dataset):
         k = MODE_TO_SPLIT[mode]
         documents = np.arange(bounds[k], bounds[k + 1])
         self.mode, self.max_seq_len, self.eos_id, self.mask_eos = mode, max_seq_len, eos_id, mask_eos
+        self.reset_position_ids = reset_position_ids
         self.name = "gpt_" + mode
         local_rank = int(os.environ.get("LOCAL_RANK", os.environ.get("PADDLE_RANK_IN_NODE", 0)))
         self.doc_idx, self.sample_idx, self.shuffle_idx = build_index_files(
@@ -230,10 +242,23 @@ class GPTDataset(torch.utils.data.Dataset):
         parts.append(self.corpus.doc_tokens(int(self.doc_idx[d1]), 0, int(o1) + 1))
         return np.concatenate(parts)
 
+    def _piece_lengths(self, idx: int) -> List[int]:
+        """Lengths of the document pieces that ``_tokens(idx)`` concatenates."""
+        d0, o0 = (int(x) for x in self.sample_idx[idx])
+        d1, o1 = (int(x) for x in self.sample_idx[idx + 1])
+        if d0 == d1:
+            return [o1 + 1 - o0]
+        lens = self.corpus.lens
+        return [int(lens[self.doc_idx[d0]]) - o0] + [int(lens[self.doc_idx[d]]) for d in range(d0 + 1, d1)] + [o1 + 1]
+
     def __getitem__(self, index: int):
-        seq = self._tokens(int(self.shuffle_idx[index])).astype(np.int64)
+        idx = int(self.shuffle_idx[index])
+        seq = self._tokens(idx).astype(np.int64)
         tokens, labels = seq[:-1], seq[1:]
-        position_ids = np.arange(len(tokens), dtype=np.int64)
+        if self.reset_position_ids:
+            position_ids = document_positions(self._piece_lengths(idx), len(tokens))
+        else:
+            position_ids = np.arange(len(tokens), dtype=np.int64)
         if self.mode == "Test":
             return [tokens, position_ids]
         loss_mask = np.ones(len(tokens), dtype=np.float32)
@@ -243,11 +268,26 @@ class GPTDataset(torch.utils.data.Dataset):
 
 
 class SyntheticGPTDataset(torch.utils.data.Dataset):
-    """Uniform-random token ids with the GPTDataset sample contract; deterministic per index."""
+    """Uniform-random token ids with the GPTDataset sample contract; deterministic per index.  ``document_length`` > 0 packs each sample
+    from documents of seeded random lengths in ``[ceil(L / 2), L + L // 2]``; with ``reset_position_ids`` their position ids restart at
+    every document (see ``GPTDataset``)."""
 
     def __init__(self, max_seq_len: int = 1024, vocab_size: int = 50304, num_samples: int = 1 << 20, mode: str = "Train", seed: int = 1234,
-                 eos_id: int = 50256, **unused):
+                 eos_id: int = 50256, reset_position_ids: bool = False, document_length: int = 0, **unused):
         self.max_seq_len, self.vocab_size, self.num_samples, self.mode, self.seed = max_seq_len, vocab_size, int(num_samples), mode, seed
+        self.reset_position_ids, self.document_length = reset_position_ids, int(document_length or 0)
+
+    def document_lengths(self, index: int) -> List[int]:
+        """The lengths of the documents packed into sample ``index`` (one document when ``document_length`` is 0)."""
+        n, L = self.max_seq_len + 1, self.document_length
+        if L <= 0:
+            return [n]
+        rng = np.random.default_rng([self.seed, index, 1])
+        lens = rng.integers(-(-L // 2), L + L // 2 + 1, size=n // max(1, -(-L // 2)) + 1)
+        cut = int(np.searchsorted(np.cumsum(lens), n))
+        lens = lens[:cut + 1].tolist()
+        lens[-1] = n - sum(lens[:-1])
+        return lens
 
     def __len__(self) -> int:
         return self.num_samples
@@ -256,7 +296,10 @@ class SyntheticGPTDataset(torch.utils.data.Dataset):
         rng = np.random.default_rng(self.seed * 1000003 + index)
         seq = rng.integers(0, self.vocab_size, size=self.max_seq_len + 1, dtype=np.int64)
         tokens, labels = seq[:-1], seq[1:]
-        position_ids = np.arange(self.max_seq_len, dtype=np.int64)
+        if self.reset_position_ids:
+            position_ids = document_positions(self.document_lengths(index), self.max_seq_len)
+        else:
+            position_ids = np.arange(self.max_seq_len, dtype=np.int64)
         if self.mode == "Test":
             return [tokens, position_ids]
         return [tokens, position_ids, labels, np.ones(self.max_seq_len, dtype=np.float32)]

@@ -16,6 +16,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from ....ops import attention as ATT
 from ....ops import functional as OF
 from ....parallel.tp_layers import parallel_matmul
 from . import model as gpt
@@ -144,8 +145,13 @@ class GPTForGeneration(nn.Module):
         causal = torch.ones(prompt_len, prompt_len, dtype=torch.bool, device=dev).tril()
         mask = (causal.unsqueeze(0) & valid.unsqueeze(1)).unsqueeze(1)                 # [b,1,s,s] bool (True = attend)
         mask = mask | torch.eye(prompt_len, dtype=torch.bool, device=dev)              # padded rows still need one key
-        # unpadded prompts (the common serving case) need no explicit mask: plain causal attention runs on the native flash kernel
-        prefill_mask = None if (attention_mask is None and bool(valid.all())) else _to_additive(mask, hidden_dtype(self.gpt))
+        # unpadded prompts (the common serving case) need no explicit mask: plain causal attention runs on the native flash kernel;
+        # left-padded ones run it too, under a document mask (see _left_padded_mask)
+        prefill_mask = None
+        if not (attention_mask is None and bool(valid.all())):
+            prefill_mask = _left_padded_mask(valid)
+            if prefill_mask is None:
+                prefill_mask = _to_additive(mask, hidden_dtype(self.gpt))
         hidden = self.gpt(input_ids, pos, prefill_mask, caches)
         logits = self._lm_logits(hidden[:, -1:, :])[:, 0, :].float()
 
@@ -254,6 +260,17 @@ GPTForGeneration._graph_state, GPTForGeneration._decode_static, GPTForGeneration
 
 def hidden_dtype(model: gpt.GPTModel):
     return model.decoder.norm.weight.dtype
+
+
+def _left_padded_mask(valid: torch.Tensor) -> Optional[ATT.DocumentMask]:
+    """The prefill mask ``causal & valid | eye`` of a LEFT-padded batch as a document mask: a valid query attends from its row's first
+    valid key, a padding query only itself (key_start = i).  ``None`` for any other validity pattern (right or interior padding)."""
+    s = valid.shape[1]
+    if s > 1 and not bool((valid[:, 1:] >= valid[:, :-1]).all()):
+        return None
+    i = torch.arange(s, device=valid.device)
+    first = s - valid.sum(-1, keepdim=True)
+    return ATT.DocumentMask.from_key_start(torch.where(valid, first, i))
 
 
 def _to_additive(bool_mask: torch.Tensor, dtype) -> torch.Tensor:

@@ -20,6 +20,8 @@ along the output rows, tensor parallelism shards it like any column-parallel wei
 With ``ffn_activation="swiglu"`` the FFN is h = silu(x W_g + b_g) * (x W_u + b_u) of width F = ``ffn_hidden_size``, and ``linear1`` is
 ``[2F, H]`` with pair-interleaved rows: row 2i is gate channel i, row 2i + 1 its up channel (the bias likewise).  A contiguous
 column-parallel shard then holds whole pairs, so tensor parallelism and checkpoint resharding split ``linear1`` as before.
+With ``reset_attention_mask`` a sample packed from several documents attends within each document only: ``GPTModel.forward`` builds
+one ``DocumentMask`` from the position ids (which restart at 0 at each document start) and every layer receives it as ``attn_mask``.
 """
 from __future__ import annotations
 
@@ -206,6 +208,13 @@ class MultiHeadAttention(nn.Module):
     def _core(self, q, k, v, attn_mask):
         scale = 1.0 / math.sqrt(self.head_dim)
         p = self.attn_dropout if self.training else 0.0
+        if isinstance(attn_mask, ATT.DocumentMask):
+            if self.use_flash_attn:
+                if p > 0:
+                    with get_rng_state_tracker().rng_state("local_seed"):
+                        return ATT.attention(q, k, v, dropout_p=p, scale=scale, attn_mask=attn_mask)
+                return ATT.attention(q, k, v, dropout_p=0.0, scale=scale, attn_mask=attn_mask)
+            attn_mask = attn_mask.additive()
         if (q.shape[1] == 1 and p == 0.0 and q.is_cuda and not torch.is_grad_enabled() and attn_mask is not None and attn_mask.dtype == q.dtype
                 and attn_mask.shape[-1] == k.shape[1] and attn_mask.numel() == q.shape[0] * k.shape[1] and k.is_contiguous() and v.is_contiguous()
                 and self.head_dim in (64, 128) and q.dtype in (torch.bfloat16, torch.float16) and OF.native_available()):
@@ -267,8 +276,9 @@ class MultiHeadAttention(nn.Module):
                 positions: Optional[torch.Tensor] = None):
         if self.cp_group is not None and cache is None:
             return self._forward_context_parallel(x, attn_mask, positions)
-        if (self.fuse_attn_qkv and self.use_flash_attn and not self.use_rope and cache is None and attn_mask is None and x.is_cuda
-                and not (self.recompute_core and self.training)):
+        doc = attn_mask if isinstance(attn_mask, ATT.DocumentMask) else None
+        if (self.fuse_attn_qkv and self.use_flash_attn and not self.use_rope and cache is None and (attn_mask is None or doc is not None)
+                and x.is_cuda and not (self.recompute_core and self.training)):
             # fused projection output [.., heads, 3, d] goes to the flash kernels as it is: q / k / v are read in place (TMA views), the
             # backward writes one packed gradient — no unbind / transpose / cat copies around the attention
             mix = self._packed_view(self.qkv_proj(x))
@@ -279,14 +289,14 @@ class MultiHeadAttention(nn.Module):
                 scale = 1.0 / math.sqrt(self.head_dim)
                 if p > 0:
                     with get_rng_state_tracker().rng_state("local_seed"):
-                        out = ATT.flash_attention_packed(mix, causal=True, dropout_p=p, scale=scale)
+                        out = ATT.flash_attention_packed(mix, causal=True, dropout_p=p, scale=scale, doc=doc)
                 else:
-                    out = ATT.flash_attention_packed(mix, causal=True, dropout_p=0.0, scale=scale)
+                    out = ATT.flash_attention_packed(mix, causal=True, dropout_p=0.0, scale=scale, doc=doc)
             else:
                 out = None
             if out is None:
                 q, k, v = self._split_packed(mix)
-                out = self._core(q, k, v, None)
+                out = self._core(q, k, v, doc)
             out = out.reshape(out.shape[0], out.shape[1], self.local_heads * self.head_dim)
             if self.sequence_parallel:
                 out = out.transpose(0, 1).contiguous()
@@ -462,14 +472,15 @@ class GPTModel(nn.Module):
                  fused_linear: bool = False, fuse_attn_qkv: bool = True, scale_qk_by_layer_num: bool = True,
                  sequence_parallel: bool = False, use_flash_attn: bool = True, fused_softmax_with_triangular: bool = True,
                  mp_group=None, moe_configs: Optional[dict] = None, fused_tp_comm: bool = False, use_rope: bool = False,
-                 normalization: Optional[str] = None, num_key_value_heads: Optional[int] = None, ffn_activation: str = "gelu", dtype=None,
-                 device=None, **unused):
+                 normalization: Optional[str] = None, num_key_value_heads: Optional[int] = None, ffn_activation: str = "gelu",
+                 reset_attention_mask: bool = False, dtype=None, device=None, **unused):
         super().__init__()
         ffn_hidden_size = ffn_hidden_size or (swiglu_ffn_size(hidden_size) if ffn_activation == "swiglu" else 4 * hidden_size)
         recompute_granularity = recompute_granularity or "full"
         self.hidden_size, self.vocab_size, self.num_layers = hidden_size, vocab_size, num_layers
         self.initializer_range = initializer_range
         self.mp_group = mp_group
+        self.reset_attention_mask = reset_attention_mask
         self.sequence_parallel = sequence_parallel and C.group_size(mp_group) > 1
         sp = self.sequence_parallel
         self.embeddings = GPTEmbeddings(vocab_size, hidden_size, max_position_embeddings, hidden_dropout_prob, initializer_range,
@@ -502,6 +513,9 @@ class GPTModel(nn.Module):
         if position_ids is None and caches is not None and caches[0].length > 0:
             past = caches[0].length
             position_ids = torch.arange(past, past + input_ids.shape[1], device=input_ids.device).unsqueeze(0).expand_as(input_ids)
+        if self.reset_attention_mask and attention_mask is None and position_ids is not None and caches is None:
+            # one mask for every layer: on CUDA one launch derives the per-row key bounds and their per-tile min / max
+            attention_mask = ATT.DocumentMask.from_positions(position_ids)
         x = self.embeddings(input_ids, position_ids)
         x = self.decoder(x, attention_mask, caches, position_ids)
         if self.sequence_parallel:

@@ -119,7 +119,7 @@ _MODEL_KEYS = ("vocab_size", "hidden_size", "num_layers", "num_attention_heads",
                "attention_probs_dropout_prob", "max_position_embeddings", "type_vocab_size", "initializer_range", "use_recompute",
                "recompute_granularity", "no_recompute_layers", "fused_linear", "fuse_attn_qkv", "scale_qk_by_layer_num",
                "sequence_parallel", "use_flash_attn", "fused_softmax_with_triangular", "moe_configs", "use_rope", "normalization", "virtual_pp_degree",
-               "num_key_value_heads", "ffn_activation")
+               "num_key_value_heads", "ffn_activation", "reset_attention_mask")
 
 
 def model_kwargs(config) -> dict:

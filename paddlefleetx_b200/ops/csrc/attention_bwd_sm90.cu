@@ -76,6 +76,7 @@ struct BwParams {
   float inv_keep;
   uint64_t seed;
   int G, gs_q;                         // grouped-query instantiation only: query heads per K/V head, q stride between groups
+  AttnDocMask doc;                     // document-mask instantiation only
 };
 
 __device__ __forceinline__ void tma_tile(const CUtensorMap* m, bool swapped, uint32_t bar, uint32_t dst, int col, int s, int b) {
@@ -86,7 +87,10 @@ __device__ __forceinline__ void tma_tile(const CUtensorMap* m, bool swapped, uin
 // so the multi-head kernels are compiled exactly as without it).  The CTA then owns a key tile of one (batch, K/V head) and walks the
 // query tiles of all G heads of the group in turn, with each head's lse / delta, dropout key, Q column and dQ column, while dK / dV
 // stay in registers: they are exact sums written once, with no atomics, and deterministic.
-template <int kHd, bool kBf16, bool kGqa>
+// kDoc (causal, Sq == Sk): query i attends keys [doc.key_start[b, i], i].  A query tile whose tile_min lies past the key tile's last key
+// holds no pair of it: the producer does not load it and the consumers do not wait for it (both skip by the same rule, for every head of
+// a group).  The ring slots count only the tiles that run.  key_start need not be monotone: the rule uses the tile's minimum.
+template <int kHd, bool kBf16, bool kGqa, bool kDoc = false>
 __global__ void __launch_bounds__(kBwThreads, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v,
                      const __grid_constant__ CUtensorMap tmap_do, const __grid_constant__ CUtensorMap tmap_dq, const __grid_constant__ BwParams prm) {
@@ -121,6 +125,13 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
   // iteration it -> (query head, first query): the query tiles of the group's first head, then the next head's, ...
   auto iter_head = [&](int it) { return kGqa ? h * prm.G + it / n_head_iter : h; };
   auto iter_q0 = [&](int it) { return (i_begin + (kGqa ? it % n_head_iter : it)) * kQt; };
+  // kDoc: the tile bounds of iteration it + 1 are loaded while iteration it runs, which keeps their latency off the loop
+  struct DocBounds { int lo, hi; };
+  auto doc_bounds = [&](int it) -> DocBounds {
+    if (!kDoc || it >= n_iter) return DocBounds{0, 0};
+    const size_t o = (size_t)b * n_q_tiles + iter_q0(it) / kQt;
+    return DocBounds{__ldg(prm.doc.tile_min + o), __ldg(prm.doc.tile_max + o)};
+  };
 
   if (warp == 4 && elect_one()) {
     tma_prefetch_desc(&tmap_q); tma_prefetch_desc(&tmap_k); tma_prefetch_desc(&tmap_v); tma_prefetch_desc(&tmap_do); tma_prefetch_desc(&tmap_dq);
@@ -138,11 +149,18 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
         tma_tile(&tmap_k, prm.swapped & 2u, kv_full, s_k + p * 8192, h * prm.hs_k + p * 64, k0, b);
         tma_tile(&tmap_v, prm.swapped & 4u, kv_full, s_v + p * 8192, h * prm.hs_v + p * 64, k0, b);
       }
+      int n_run = 0;                                  // kDoc: query tiles loaded so far (the ring slot)
+      DocBounds nxt = doc_bounds(0);
       for (int it = 0; it < n_iter; ++it) {
-        const int st = it % S::kStages, q0 = iter_q0(it);
+        const int q0 = iter_q0(it);
+        const DocBounds cur = nxt;
+        if constexpr (kDoc) nxt = doc_bounds(it + 1);
+        if (kDoc && cur.lo > k0 + kKv - 1) continue;
+        const int slot = kDoc ? n_run++ : it;
+        const int st = slot % S::kStages;
         const int hq = iter_head(it);
         const int q_col = kGqa ? h * prm.gs_q + (hq - h * prm.G) * prm.hs_q : h * prm.hs_q;
-        mbar_wait(q_empty(st), (((uint32_t)(it / S::kStages)) & 1u) ^ 1u);
+        mbar_wait(q_empty(st), (((uint32_t)(slot / S::kStages)) & 1u) ^ 1u);
         mbar_arrive_expect_tx(q_full(st), 2 * S::kQBytes + S::kStatBytes);
         for (int p = 0; p < kPanels; ++p) {
           tma_tile(&tmap_q, prm.swapped & 1u, q_full(st), s_q + st * S::kQBytes + p * 8192, q_col + p * 64, q0, b);
@@ -168,13 +186,19 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
 #pragma unroll
     for (int i = 0; i < kHd / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
     mbar_wait(kv_full, 0);
+    int n_run = 0;
+    DocBounds nxt = doc_bounds(0);
     for (int it = 0; it < n_iter; ++it) {
-      const int st = it % S::kStages;
       const int q0 = iter_q0(it);
+      const DocBounds cur = nxt;
+      if constexpr (kDoc) nxt = doc_bounds(it + 1);
+      if (kDoc && cur.lo > k0 + kKv - 1) continue;   // never the diagonal tile i_begin (its tile_min <= its first query = k0)
+      const int slot = kDoc ? n_run++ : it;
+      const int st = slot % S::kStages;
       const int hq = iter_head(it);
       if (kGqa && it != 0 && q0 == i_begin * kQt) key = attn_rng_key(prm.seed, (uint32_t)(b * prm.H + hq));   // next head of the group
       const uint32_t sq = s_q + st * S::kQBytes, sdo = s_do + st * S::kQBytes;
-      mbar_wait(q_full(st), ((uint32_t)(it / S::kStages)) & 1u);
+      mbar_wait(q_full(st), ((uint32_t)(slot / S::kStages)) & 1u);
       float s[kQt / 2], dp[kQt / 2];                                  // [4 g + e]: key k_row + 8 (e / 2), query 8 g + col_in8 + (e % 2)
       wgmma_fence();
 #pragma unroll
@@ -192,7 +216,8 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
       const float* lse_s = reinterpret_cast<const float*>(smem_gen + (s_stat - smem_base) + st * S::kStatBytes);
       const float* dl_s = lse_s + kQt;
       // masks are decided per tile (warp-uniform branches): only diagonal / ragged tiles pay per-element compares
-      const bool tile_mask = (prm.causal && (k0 + kKv - 1 > q0 + off)) || (k0 + kKv > prm.Sk);
+      const bool tile_mask = (prm.causal && (k0 + kKv - 1 > q0 + off)) || (k0 + kKv > prm.Sk) ||
+                             (kDoc && k0 < cur.hi);
       uint32_t pw[kQt / 4], dsw[kQt / 4];                             // P_drop^T and dS^T as packed 16-bit pairs, in wgmma A-fragment order
 #pragma unroll
       for (int g = 0; g < kQt / 8; ++g) {
@@ -206,6 +231,11 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
           if (tile_mask) {
             if (kg >= prm.Sk || (prm.causal && kg > q0 + qc + off)) p0 = 0.f;
             if (kg >= prm.Sk || (prm.causal && kg > q0 + qc + 1 + off)) p1 = 0.f;
+            if constexpr (kDoc) {                  // rows past Sq have P = 0 already (lse2 = +inf)
+              const int* ks = prm.doc.key_start + (size_t)b * prm.Sq;
+              if (q0 + qc < prm.Sq && kg < __ldg(ks + q0 + qc)) p0 = 0.f;
+              if (q0 + qc + 1 < prm.Sq && kg < __ldg(ks + q0 + qc + 1)) p1 = 0.f;
+            }
           }
           float d0 = dp[4 * g + 2 * hh], d1 = dp[4 * g + 2 * hh + 1];
           float pd0 = p0 * p_to_pdrop, pd1 = p1 * p_to_pdrop;
@@ -347,10 +377,11 @@ bool make_map(CUtensorMap* m, const AttnView& t, int dtype, int B, int S, int H,
 
 }  // namespace
 
-template <int kHd, bool kBf16, bool kGqa>
+template <int kHd, bool kBf16, bool kGqa, bool kDoc = false>
 static cudaError_t attention_bwd_impl(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, const AttnView& dout, const float* lse,
                                       const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int Sq,
-                                      int Sk, int H, int Hkv, float scale, bool causal, AttnDropout drop, cudaStream_t st) {
+                                      int Sk, int H, int Hkv, float scale, bool causal, AttnDropout drop, cudaStream_t st,
+                                      const AttnDocMask& doc = AttnDocMask{}) {
   const int G = H / Hkv;
   constexpr int D = kHd;
   constexpr int dt = kBf16 ? 1 : 0;
@@ -384,13 +415,14 @@ static cudaError_t attention_bwd_impl(const AttnView& q, const AttnView& k, cons
   prm.drop_thresh16 = drop.p > 0.f ? (uint32_t)(drop.p * 65536.f + 0.5f) : 0u;
   prm.inv_keep = drop.p > 0.f ? 1.f / (1.f - drop.p) : 1.f;
   prm.seed = drop.seed;
+  prm.doc = doc;
   static bool attr_set = false;
   if (!attr_set) {
-    if ((e = cudaFuncSetAttribute(attention_bwd_kernel<kHd, kBf16, kGqa>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(attention_bwd_kernel<kHd, kBf16, kGqa, kDoc>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal)) != cudaSuccess) return e;
     attr_set = true;
   }
   const int n_kv = (Sk + kKv - 1) / kKv;
-  attention_bwd_kernel<kHd, kBf16, kGqa><<<(unsigned)(n_kv * B * Hkv), kBwThreads, S::kTotal, st>>>(tq, tk, tv, tdo, tdq, prm);
+  attention_bwd_kernel<kHd, kBf16, kGqa, kDoc><<<(unsigned)(n_kv * B * Hkv), kBwThreads, S::kTotal, st>>>(tq, tk, tv, tdo, tdq, prm);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   attn_bwd_dq_convert_kernel<kBf16, kGqa><<<1184, 256, 0, st>>>(dq_acc, (uint16_t*)const_cast<void*>(dq.ptr), dq.sb, dq.ss, dq.sh, B, Sq, H, kHd, G, dq.sg);
   return cudaGetLastError();
@@ -403,6 +435,24 @@ cudaError_t attention_bwd(const AttnView& q, const AttnView& k, const AttnView& 
   if (H < 1 || Hkv < 1 || H % Hkv != 0 || (Hkv < H && (q.sg % 8 || dq.sg % 8))) return cudaErrorInvalidValue;
   for (const AttnView* t : {&q, &k, &v, &out, &dout, &dq, &dk, &dv}) if (!view_ok(*t)) return cudaErrorInvalidValue;
 #define PFX_BWD(HD, BF, GQA) attention_bwd_impl<HD, BF, GQA>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, Sq, Sk, H, Hkv, scale, causal, drop, st)
+  if (Hkv < H) {
+    if (dtype == 1) return D == 128 ? PFX_BWD(128, true, true) : PFX_BWD(64, true, true);
+    return D == 128 ? PFX_BWD(128, false, true) : PFX_BWD(64, false, true);
+  }
+  if (dtype == 1) return D == 128 ? PFX_BWD(128, true, false) : PFX_BWD(64, true, false);
+  return D == 128 ? PFX_BWD(128, false, false) : PFX_BWD(64, false, false);
+#undef PFX_BWD
+}
+
+cudaError_t attention_bwd_doc(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, const AttnView& dout, const float* lse,
+                              const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int S,
+                              int H, int Hkv, int D, float scale, AttnDropout drop, const AttnDocMask& doc, int dtype, cudaStream_t st) {
+  if ((D != 64 && D != 128) || (dtype != 0 && dtype != 1) || B < 1 || S < 1) return cudaErrorInvalidValue;
+  if (H < 1 || Hkv < 1 || H % Hkv != 0 || (Hkv < H && (q.sg % 8 || dq.sg % 8))) return cudaErrorInvalidValue;
+  if (doc.key_start == nullptr || doc.tile_min == nullptr || doc.tile_max == nullptr) return cudaErrorInvalidValue;
+  for (const AttnView* t : {&q, &k, &v, &out, &dout, &dq, &dk, &dv}) if (!view_ok(*t)) return cudaErrorInvalidValue;
+#define PFX_BWD(HD, BF, GQA) \
+  attention_bwd_impl<HD, BF, GQA, true>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, S, S, H, Hkv, scale, true, drop, st, doc)
   if (Hkv < H) {
     if (dtype == 1) return D == 128 ? PFX_BWD(128, true, true) : PFX_BWD(64, true, true);
     return D == 128 ? PFX_BWD(128, false, true) : PFX_BWD(64, false, true);

@@ -17,6 +17,7 @@
 // Causal tiles above the diagonal are never loaded; masks are applied only on diagonal / ragged tiles.  Output O (the inputs' type) and the row-wise
 // log-sum-exp (fp32, [B, H, S]) are written from registers.  Reference call site: flash_attention in hybrid_model.py:284-301
 // (FlashAttention-2 library on Ampere mma.sync).
+#include <climits>
 #include <cstdio>
 
 #include "pfx_ptx.cuh"
@@ -56,12 +57,16 @@ __device__ __forceinline__ void tma3(const CUtensorMap* m, bool swapped, uint32_
 // the multi-head kernels are compiled exactly as without it); query head h loads Q at column (h / G) * gs_q + (h % G) * hs_q and K / V
 // of head h / G.  The work order keeps the heads of one batch adjacent, so the G query heads of a group stream the same K / V tiles
 // at about the same time and share them through L2.
-template <int kD, bool kCausal, bool kBf16, bool kGqa>
+// kDoc (with kCausal, Sq == Sk): query i attends keys [doc.key_start[b, i], i] (AttnDocMask).  A 64-query tile starts at key tile
+// tile_min / 128 in the producer and the consumers alike, and only tiles with key0 < tile_max (plus the diagonal / ragged ones) pay
+// per-element compares.
+template <int kD, bool kCausal, bool kBf16, bool kGqa, bool kDoc = false>
 __global__ void __launch_bounds__(kFaThreads, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v,
                      uint16_t* __restrict__ out, int64_t o_sb, int64_t o_ss, int64_t o_sh, float* __restrict__ lse, int B, int Sq, int Sk, int H,
                      float scale_log2, int hs_q, int hs_k, int hs_v, uint32_t swapped, uint32_t drop_thresh16, float inv_keep, uint64_t seed,
-                     int G, int gs_q) {
+                     int G, int gs_q, AttnDocMask doc) {
+  static_assert(!kDoc || kCausal, "the document mask is a causal mask with a per-row lower key bound");
   using S = FaSmem<kD>;
   constexpr int kPanels = kD / 64;                 // 64-element (128-byte) column panels of a D-wide tile
   extern __shared__ uint8_t smem_raw[];
@@ -82,6 +87,9 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
   auto item_tile = [&](int w) { return n_q_tiles - 1 - w / hb_count; };
   auto tile_n_kv = [&](int q_tile) {                 // key tiles a query tile attends to
     return kCausal ? min(n_kv_all, (q_tile * kFaQ + kFaQ - 1 + (Sk - Sq)) / kFaKv + 1) : n_kv_all;
+  };
+  auto tile_j0 = [&](int q_tile, int b) {            // first key tile a query tile attends to
+    return kDoc ? __ldg(doc.tile_min + (size_t)b * n_q_tiles + q_tile) / kFaKv : 0;
   };
 
   if (warp == 4 && elect_one()) {
@@ -105,7 +113,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
         mbar_wait(q_empty, ((uint32_t)it & 1u) ^ 1u);
         mbar_arrive_expect_tx(q_full, S::kQBytes);
         for (int p = 0; p < kPanels; ++p) tma3(&tmap_q, swapped & 1u, q_full, smem_q + p * (kFaQ * 128), q_col + p * 64, q_tile * kFaQ, b);
-        for (int j = 0; j < n_kv; ++j, ++t) {
+        for (int j = tile_j0(q_tile, b); j < n_kv; ++j, ++t) {
           const int stage = t & 1;
           mbar_wait(kv_empty(stage), ((t >> 1) & 1u) ^ 1u);
           const uint32_t sk = smem_kv + stage * S::kStageBytes, sv = sk + S::kKBytes;
@@ -136,8 +144,17 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
       for (int i = 0; i < kD / 2; ++i) o[i] = 0.f;
       const uint32_t rng_key = attn_rng_key(seed, (uint32_t)(b * H + h));
       const uint32_t rng_pairs = ((uint32_t)Sk + 1u) >> 1;
+      int doc_max = 0, doc_ks[2] = {0, 0};            // kDoc: the tile's largest key_start, and that of this thread's two rows
+      if constexpr (kDoc) {
+        doc_max = __ldg(doc.tile_max + (size_t)b * n_q_tiles + q_tile);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int row_g = q0 + row_lo + 8 * hh;
+          doc_ks[hh] = row_g < Sq ? __ldg(doc.key_start + (size_t)b * Sq + row_g) : 0;
+        }
+      }
       mbar_wait(q_full, (uint32_t)it & 1u);
-      for (int j = 0; j < n_kv; ++j, ++t) {
+      for (int j = tile_j0(q_tile, b); j < n_kv; ++j, ++t) {
         const int stage = t & 1;
         const uint32_t sk = smem_kv + stage * S::kStageBytes, sv = sk + S::kKBytes;
         mbar_wait(kv_full(stage), (t >> 1) & 1u);
@@ -151,13 +168,13 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
         wgmma_commit();
         wgmma_wait<0>();
         const int key0 = j * kFaKv;
-        const bool need_mask = (kCausal && key0 + kFaKv - 1 > q0 + (Sk - Sq)) || (key0 + kFaKv > Sk);
+        const bool need_mask = (kCausal && key0 + kFaKv - 1 > q0 + (Sk - Sq)) || (key0 + kFaKv > Sk) || (kDoc && key0 < doc_max);
         if (need_mask) {
 #pragma unroll
           for (int i = 0; i < kFaKv / 2; ++i) {
             const int cg = key0 + 8 * (i >> 2) + col_in8 + (i & 1);
             const int row_g = q0 + row_lo + 8 * ((i >> 1) & 1);
-            if (cg >= Sk || (kCausal && cg > row_g + (Sk - Sq))) s[i] = -INFINITY;
+            if (cg >= Sk || (kCausal && cg > row_g + (Sk - Sq)) || (kDoc && cg < doc_ks[(i >> 1) & 1])) s[i] = -INFINITY;
           }
         }
         float f[2], m_use[2];
@@ -226,9 +243,9 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
   }
 }
 
-template <int kD, bool kCausal, bool kBf16, bool kGqa>
+template <int kD, bool kCausal, bool kBf16, bool kGqa, bool kDoc = false>
 cudaError_t launch_fa(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H, int Hkv,
-                      float scale, AttnDropout drop, cudaStream_t st) {
+                      float scale, AttnDropout drop, cudaStream_t st, AttnDocMask doc = AttnDocMask{}) {
   using S = FaSmem<kD>;
   CUtensorMap tq, tk, tv;
   bool sq = false, sk = false, sv = false;
@@ -241,7 +258,7 @@ cudaError_t launch_fa(const AttnView& q, const AttnView& k, const AttnView& v, c
   ok &= make_tmap_bshd(&tk, k.ptr, dt, inner(k), Sk, B, (uint64_t)k.ss * 2, (uint64_t)k.sb * 2, 64, kFaKv, &sk);
   ok &= make_tmap_bshd(&tv, v.ptr, dt, inner(v), Sk, B, (uint64_t)v.ss * 2, (uint64_t)v.sb * 2, 64, 64, &sv);
   if (!ok) return cudaErrorInvalidValue;
-  auto kern = attention_fwd_kernel<kD, kCausal, kBf16, kGqa>;
+  auto kern = attention_fwd_kernel<kD, kCausal, kBf16, kGqa, kDoc>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal);
@@ -259,7 +276,7 @@ cudaError_t launch_fa(const AttnView& q, const AttnView& k, const AttnView& v, c
   const float inv_keep = drop.p > 0.f ? 1.f / (1.f - drop.p) : 1.f;
   const uint32_t swapped = (sq ? 1u : 0u) | (sk ? 2u : 0u) | (sv ? 4u : 0u);
   kern<<<grid, kFaThreads, S::kTotal, st>>>(tq, tk, tv, (uint16_t*)const_cast<void*>(out.ptr), out.sb, out.ss, out.sh, lse, B, Sq, Sk, H,
-                                            scale * 1.4426950408889634f, (int)q.sh, (int)k.sh, (int)v.sh, swapped, thresh, inv_keep, drop.seed, G, (int)q.sg);
+                                            scale * 1.4426950408889634f, (int)q.sh, (int)k.sh, (int)v.sh, swapped, thresh, inv_keep, drop.seed, G, (int)q.sg, doc);
   return cudaGetLastError();
 }
 
@@ -270,6 +287,13 @@ cudaError_t launch_fa_dt(const AttnView& q, const AttnView& k, const AttnView& v
                               : launch_fa<128, false, kBf16, kGqa>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, scale, drop, st);
   return causal ? launch_fa<64, true, kBf16, kGqa>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, scale, drop, st)
                 : launch_fa<64, false, kBf16, kGqa>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, scale, drop, st);
+}
+
+template <bool kBf16, bool kGqa>
+cudaError_t launch_fa_doc(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int S, int H, int Hkv, int D,
+                          float scale, AttnDropout drop, const AttnDocMask& doc, cudaStream_t st) {
+  if (D == 128) return launch_fa<128, true, kBf16, kGqa, true>(q, k, v, out, lse, B, S, S, H, Hkv, scale, drop, st, doc);
+  return launch_fa<64, true, kBf16, kGqa, true>(q, k, v, out, lse, B, S, S, H, Hkv, scale, drop, st, doc);
 }
 
 }  // namespace
@@ -285,6 +309,54 @@ cudaError_t attention_fwd_v2(const AttnView& q, const AttnView& k, const AttnVie
                       : launch_fa_dt<false, true>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, D, scale, causal, drop, st);
   return dtype == 1 ? launch_fa_dt<true, false>(q, k, v, out, lse, B, Sq, Sk, H, H, D, scale, causal, drop, st)
                     : launch_fa_dt<false, false>(q, k, v, out, lse, B, Sq, Sk, H, H, D, scale, causal, drop, st);
+}
+
+cudaError_t attention_fwd_doc(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int S, int H, int Hkv,
+                              int D, float scale, AttnDropout drop, const AttnDocMask& doc, int dtype, cudaStream_t st) {
+  if ((D != 64 && D != 128) || (dtype != 0 && dtype != 1) || B < 1 || S < 1) return cudaErrorInvalidValue;
+  if (H < 1 || Hkv < 1 || H % Hkv != 0 || (Hkv < H && q.sg % 8)) return cudaErrorInvalidValue;
+  if (doc.key_start == nullptr || doc.tile_min == nullptr || doc.tile_max == nullptr) return cudaErrorInvalidValue;
+  for (const AttnView* t : {&q, &k, &v, &out})
+    if (t->ptr == nullptr || (reinterpret_cast<uintptr_t>(t->ptr) % 16) || t->sb % 8 || t->ss % 8 || t->sh % 8) return cudaErrorInvalidValue;
+  if (Hkv < H)
+    return dtype == 1 ? launch_fa_doc<true, true>(q, k, v, out, lse, B, S, H, Hkv, D, scale, drop, doc, st)
+                      : launch_fa_doc<false, true>(q, k, v, out, lse, B, S, H, Hkv, D, scale, drop, doc, st);
+  return dtype == 1 ? launch_fa_doc<true, false>(q, k, v, out, lse, B, S, H, H, D, scale, drop, doc, st)
+                    : launch_fa_doc<false, false>(q, k, v, out, lse, B, S, H, H, D, scale, drop, doc, st);
+}
+
+// ---- document-mask bounds: key_start[b, i] = clamp(i - pos[b, i], 0, i) (or clamp(src, 0, i) when src already holds key starts), and
+// the minimum / maximum of key_start over every 64-query tile.  One 64-thread block per (tile, b).
+__global__ void attn_doc_bounds_kernel(const int64_t* __restrict__ src, int from_positions, int S, int n_tiles, int* __restrict__ key_start,
+                                       int* __restrict__ tile_min, int* __restrict__ tile_max) {
+  __shared__ int red[2][2];
+  const int b = blockIdx.y, i = blockIdx.x * 64 + threadIdx.x;
+  int lo = INT_MAX, hi = 0;
+  if (i < S) {
+    const int64_t x = src[(size_t)b * S + i];
+    const int64_t ks = from_positions ? (int64_t)i - x : x;
+    const int v = (int)(ks < 0 ? 0 : (ks > i ? i : ks));
+    key_start[(size_t)b * S + i] = v;
+    lo = hi = v;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    lo = min(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+    hi = max(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+  }
+  if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = lo; red[1][threadIdx.x >> 5] = hi; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    tile_min[(size_t)b * n_tiles + blockIdx.x] = min(red[0][0], red[0][1]);
+    tile_max[(size_t)b * n_tiles + blockIdx.x] = max(red[1][0], red[1][1]);
+  }
+}
+
+cudaError_t attention_doc_bounds(const int64_t* src, bool from_positions, int B, int S, int* key_start, int* tile_min, int* tile_max, cudaStream_t st) {
+  if (src == nullptr || B < 1 || S < 1 || B > 65535) return cudaErrorInvalidValue;
+  const int n_tiles = (S + 63) / 64;
+  attn_doc_bounds_kernel<<<dim3(n_tiles, B), 64, 0, st>>>(src, from_positions ? 1 : 0, S, n_tiles, key_start, tile_min, tile_max);
+  return cudaGetLastError();
 }
 
 cudaError_t attention_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int Sq, int Sk, int H, int D, float scale,

@@ -883,6 +883,75 @@ void attention_bwd(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v
                                     causal, pfx::AttnDropout{(float)dropout_p, (uint64_t)seed}, dtype_code(q), cur_stream()));
 }
 
+// Document-mask bounds from int64 [B, S] position ids (from_positions: key_start = clamp(i - pos, 0, i)) or key starts (clamped into
+// [0, i]): returns (key_start int32 [B, S], tile_min, tile_max int32 [B, ceil(S / 64)]), computed by one kernel.
+std::vector<at::Tensor> attention_doc_bounds(const at::Tensor& src, bool from_positions) {
+  TORCH_CHECK(src.is_cuda() && src.dim() == 2 && src.is_contiguous() && src.scalar_type() == at::kLong, "attention_doc_bounds: int64 [B, S] CUDA tensor");
+  TORCH_CHECK(src.size(0) >= 1 && src.size(0) <= 65535 && src.size(1) >= 1, "attention_doc_bounds: 1 <= B <= 65535 and S >= 1");
+  const c10::cuda::CUDAGuard guard(src.device());
+  const int64_t B = src.size(0), S = src.size(1), T = (S + 63) / 64;
+  auto i32 = src.options().dtype(at::kInt);
+  auto ks = at::empty({B, S}, i32), tmin = at::empty({B, T}, i32), tmax = at::empty({B, T}, i32);
+  PFX_CUDA_CHECK(pfx::attention_doc_bounds(src.data_ptr<int64_t>(), from_positions, (int)B, (int)S, ks.data_ptr<int>(), tmin.data_ptr<int>(),
+                                           tmax.data_ptr<int>(), cur_stream()));
+  return {ks, tmin, tmax};
+}
+
+static pfx::AttnDocMask attn_doc(const at::Tensor& ks, const at::Tensor& tmin, const at::Tensor& tmax, int64_t B, int64_t S, const char* fn) {
+  const int64_t T = (S + 63) / 64;
+  for (const at::Tensor* t : {&ks, &tmin, &tmax})
+    TORCH_CHECK(t->is_cuda() && t->is_contiguous() && t->scalar_type() == at::kInt, fn, ": document bounds must be contiguous int32 CUDA tensors");
+  TORCH_CHECK(ks.numel() == B * S && tmin.numel() == B * T && tmax.numel() == B * T, fn, ": document bounds must be [B, S] and [B, ceil(S / 64)]");
+  return pfx::AttnDocMask{ks.data_ptr<int>(), tmin.data_ptr<int>(), tmax.data_ptr<int>()};
+}
+
+// Causal flash attention under a document mask (self-attention, Sq == Sk): query i attends keys [key_start[b, i], i].  The bounds come
+// from attention_doc_bounds.  Views as in attention_fwd_v2.
+std::vector<at::Tensor> attention_fwd_doc(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v, const at::Tensor& key_start,
+                                          const at::Tensor& tile_min, const at::Tensor& tile_max, double scale, double dropout_p, int64_t seed) {
+  const int64_t Hkv = attn_kv_heads(q, k, "attention_fwd_doc");
+  const int64_t H = attn_q_heads(q), D = q.size(q.dim() - 1);
+  TORCH_CHECK(k.sizes() == v.sizes() && q.size(0) == k.size(0) && q.size(1) == k.size(1) && D == k.size(3),
+              "attention_fwd_doc: shape mismatch (self-attention: q and k have one sequence length)");
+  TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type(), "attention_fwd_doc: q, k, v must have one dtype");
+  const pfx::AttnDocMask doc = attn_doc(key_start, tile_min, tile_max, q.size(0), q.size(1), "attention_fwd_doc");
+  const c10::cuda::CUDAGuard guard(q.device());
+  auto out = at::empty({q.size(0), q.size(1), H, D}, q.options());
+  auto lse = at::empty({q.size(0), H, q.size(1)}, q.options().dtype(at::kFloat));
+  PFX_CUDA_CHECK(pfx::attention_fwd_doc(attn_qview(q, "q", Hkv), attn_view(k, "k"), attn_view(v, "v"), attn_view(out, "out"), lse.data_ptr<float>(),
+                                        (int)q.size(0), (int)q.size(1), (int)H, (int)Hkv, (int)D, (float)scale,
+                                        pfx::AttnDropout{(float)dropout_p, (uint64_t)seed}, doc, dtype_code(q), cur_stream()));
+  return {out, lse};
+}
+
+// Backward of attention_fwd_doc: writes dq / dk / dv into the given (possibly strided) views.
+void attention_bwd_doc(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v, const at::Tensor& out, const at::Tensor& dout, const at::Tensor& lse,
+                       at::Tensor& dq, at::Tensor& dk, at::Tensor& dv, const at::Tensor& key_start, const at::Tensor& tile_min, const at::Tensor& tile_max,
+                       double scale, double dropout_p, int64_t seed) {
+  const int64_t Hkv = attn_kv_heads(q, k, "attention_bwd_doc");
+  const int64_t H = attn_q_heads(q), D = q.size(q.dim() - 1);
+  TORCH_CHECK(D == 128 || D == 64, "attention_bwd_doc: head_dim must be 64 or 128");
+  TORCH_CHECK(k.sizes() == v.sizes() && q.size(0) == k.size(0) && q.size(1) == k.size(1) && D == k.size(3), "attention_bwd_doc: k / v shape mismatch");
+  TORCH_CHECK(k.sizes() == dk.sizes() && k.sizes() == dv.sizes(), "attention_bwd_doc: dk / dv must have the shape of k");
+  TORCH_CHECK(q.sizes() == dq.sizes(), "attention_bwd_doc: dq must have the shape of q");
+  const std::vector<int64_t> o_shape{q.size(0), q.size(1), H, D};
+  TORCH_CHECK(out.sizes() == at::IntArrayRef(o_shape) && dout.sizes() == at::IntArrayRef(o_shape), "attention_bwd_doc: out / dout must be [B,S,H,D]");
+  TORCH_CHECK(lse.is_cuda() && lse.is_contiguous() && lse.scalar_type() == at::kFloat && lse.numel() == q.size(0) * q.size(1) * H, "attention_bwd_doc: lse");
+  for (const at::Tensor* t : std::initializer_list<const at::Tensor*>{&k, &v, &out, &dout, &dq, &dk, &dv})
+    TORCH_CHECK(t->scalar_type() == q.scalar_type(), "attention_bwd_doc: q, k, v, out, dout and the gradients must have one dtype");
+  const pfx::AttnDocMask doc = attn_doc(key_start, tile_min, tile_max, q.size(0), q.size(1), "attention_bwd_doc");
+  const c10::cuda::CUDAGuard guard(q.device());
+  const int64_t B = q.size(0), S = q.size(1);
+  const int64_t s_pad = (S + 63) / 64 * 64;
+  auto f32 = q.options().dtype(at::kFloat);
+  auto dq_acc = at::empty({B, S, H, D}, f32);
+  auto stats = at::empty({2, B * H * s_pad}, f32);
+  PFX_CUDA_CHECK(pfx::attention_bwd_doc(attn_qview(q, "q", Hkv), attn_view(k, "k"), attn_view(v, "v"), attn_view(out, "out"), attn_view(dout, "dout"),
+                                        lse.data_ptr<float>(), attn_qview(dq, "dq", Hkv), attn_view(dk, "dk"), attn_view(dv, "dv"), dq_acc.data_ptr<float>(),
+                                        stats[0].data_ptr<float>(), stats[1].data_ptr<float>(), (int)B, (int)S, (int)H, (int)Hkv, (int)D, (float)scale,
+                                        pfx::AttnDropout{(float)dropout_p, (uint64_t)seed}, doc, dtype_code(q), cur_stream()));
+}
+
 at::Tensor attention_decode_packed(const at::Tensor& qkv, at::Tensor& k, at::Tensor& v, c10::optional<at::Tensor> mask, const at::Tensor& write_idx,
                                    double scale) {
   // qkv [B,1,Hkv,G+2,D] (fused projection output: per K/V head its G queries, key and value; G = 1 is [B,1,H,3,D]); appends this step's
@@ -1137,6 +1206,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("embedding_bwd_max_tokens", &embedding_bwd_max_tokens);
   m.def("attention_fwd_v2", &attention_fwd_v2);
   m.def("attention_bwd", &attention_bwd);
+  m.def("attention_doc_bounds", &attention_doc_bounds);
+  m.def("attention_fwd_doc", &attention_fwd_doc);
+  m.def("attention_bwd_doc", &attention_bwd_doc);
   m.def("attention_decode", &attention_decode);
   m.def("attention_decode_packed", &attention_decode_packed);
   m.def("gemm_bias_gelu_dual", &gemm_bias_gelu_dual);

@@ -29,12 +29,34 @@ struct AttnDropout {
 cudaError_t attention_fwd_v2(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H,
                              int Hkv, int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st);
 
+// Intra-document causal mask for packed sequences (self-attention, Sq == Sk == S): query i of batch row b attends the keys
+// [key_start[b, i], i], with 0 <= key_start[b, i] <= i.  tile_min / tile_max hold the minimum / maximum of key_start over each
+// 64-query tile ([B, ceil(S / 64)]); the kernels skip whole key tiles from them and compare per element only on boundary tiles.
+struct AttnDocMask {
+  const int* key_start;     // int32 [B, S]
+  const int* tile_min;      // int32 [B, ceil(S / 64)]
+  const int* tile_max;
+};
+
+// Writes key_start = clamp(i - src[b, i], 0, i) when from_positions (src = position ids, which restart at 0 at each document), or
+// clamp(src[b, i], 0, i) otherwise, and the per-tile bounds of AttnDocMask.  src int64 [B, S].
+cudaError_t attention_doc_bounds(const int64_t* src, bool from_positions, int B, int S, int* key_start, int* tile_min, int* tile_max, cudaStream_t st);
+
+// attention_fwd_v2 with causal = true under a document mask (separate kernel instantiations).
+cudaError_t attention_fwd_doc(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int S, int H, int Hkv,
+                              int D, float scale, AttnDropout drop, const AttnDocMask& doc, int dtype, cudaStream_t st);
+
 // Backward.  Workspace: dq_acc fp32 [B, Sq, H, D] (zeroed by the call), lse2 / delta fp32 [B, H, round_up(Sq, 64)].
 // dq / dk / dv may be strided views (e.g. slices of one packed [B, S, H, 3, D] gradient buffer).  D is 64 or 128; dtype as above.
 // With Hkv < H one CTA per (batch, K/V head, key tile) walks the query tiles of every head of the group, so dk / dv are written once.
 cudaError_t attention_bwd(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, const AttnView& dout, const float* lse,
                           const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int Sq,
                           int Sk, int H, int Hkv, int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st);
+
+// attention_bwd with causal = true under a document mask: a key tile skips every query tile whose tile_min lies past its last key.
+cudaError_t attention_bwd_doc(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, const AttnView& dout, const float* lse,
+                              const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int S,
+                              int H, int Hkv, int D, float scale, AttnDropout drop, const AttnDocMask& doc, int dtype, cudaStream_t st);
 
 // Evoformer gated attention (head width 32, H even): softmax(scale QK^T + mask_bias[g, k] + pair_bias[g / groups_per_pair, h, q, k]) V * sigmoid(gate).
 // q / out / gate [G, Sq, H, 32], k / v [G, Sk, H, 32] bf16 contiguous; mask_bias fp32 [G, Sk]; pair_bias bf16; stats fp32 [2, G, H, Sq]: the

@@ -54,6 +54,23 @@ def check_ffn_activation(m, d, compress) -> None:
                          "tensor parallelism shards whole gate / up pairs")
 
 
+def check_document_mask(m, d, data) -> None:
+    """``Model.reset_attention_mask`` (attention stays inside each packed document) needs ``Data.*.dataset.reset_position_ids``, which
+    produces the position ids the mask is derived from, and a layout whose attention sees whole sequences with their positions."""
+    if not m.get("reset_attention_mask", False):
+        return
+    sets = [data[k].get("dataset", {}) or {} for k in ("Train", "Eval") if data.get(k)]
+    if not sets or not all(ds.get("reset_position_ids", False) for ds in sets):
+        raise ValueError("Model.reset_attention_mask needs Data.*.dataset.reset_position_ids: true (without restarting positions the "
+                         "document mask would silently be plain causal)")
+    if d.get("pp_degree", 1) > 1:
+        raise ValueError("Model.reset_attention_mask is not supported with pipeline parallelism (Distributed.pp_degree > 1): "
+                         "later stages receive no position ids")
+    if d.get("cp_degree", 1) > 1:
+        raise ValueError("Model.reset_attention_mask is not supported with context parallelism (Distributed.cp_degree > 1): "
+                         "the ring and Ulysses layouts shard the sequence")
+
+
 def check_config(cfg):
     g, d = cfg.Global, cfg.get("Distributed", {})
     for key in ("local_batch_size", "micro_batch_size"):
@@ -73,5 +90,6 @@ def check_config(cfg):
         raise ValueError("num_attention_heads must be divisible by mp_degree")
     check_kv_heads(m, d, cfg.get("Compress", {}) or {})
     check_ffn_activation(m, d, cfg.get("Compress", {}) or {})
+    check_document_mask(m, d, cfg.get("Data", {}) or {})
     logger.debug("config checks passed")
     return True

@@ -5,6 +5,8 @@
     ernie  ERNIE 10B-class encoder, mp x ZeRO stage 3                                                        (tokens/s)
     gpt-1.3b    GPT 1.3B (tanh-GELU FFN, 4h), data parallel, 8 x 1024 tokens / GPU                          (tokens/s)
     gpt-swiglu  the same model with the SwiGLU FFN (Model.ffn_activation: swiglu, F = 5632)                  (tokens/s)
+    gpt-1.3b-docs  GPT 1.3B on rows packed from documents of 128 to 383 tokens (seeded lengths, mean 256),
+                intra-document attention (Model.reset_attention_mask)                                          (tokens/s)
 
 Synthetic data of the named shape, random-init weights, bf16.  Same contract as bench.py: W warm-up steps, K steps timed with CUDA
 events between barriers, max over ranks, nvidia-smi clocks / throttle reasons sampled during the timed region, the exposed-
@@ -29,7 +31,7 @@ CFG = os.path.join(ROOT, "paddlefleetx_b200", "configs")
 
 def parse():
     p = argparse.ArgumentParser()
-    p.add_argument("--workload", required=True, choices=["moe", "vit", "ernie", "gpt-1.3b", "gpt-swiglu"])
+    p.add_argument("--workload", required=True, choices=["moe", "vit", "ernie", "gpt-1.3b", "gpt-swiglu", "gpt-1.3b-docs"])
     p.add_argument("--gpus", type=int, default=1)
     p.add_argument("--steps", type=int, default=5)
     p.add_argument("--warmup", type=int, default=3)
@@ -59,14 +61,16 @@ def main():
     dev = torch.device("cuda", torch.cuda.current_device())
     common = ["Engine.max_steps=1000000", "Engine.eval_freq=-1", "Engine.logging_freq=1000000", "Engine.save_load.save_steps=-1",
               "Engine.mix_precision.enable=True", "Engine.mix_precision.dtype=bfloat16", "Global.global_batch_size=None"]
-    if a.workload in ("gpt-1.3b", "gpt-swiglu"):
+    if a.workload in ("gpt-1.3b", "gpt-swiglu", "gpt-1.3b-docs"):
         local = a.local_batch or 8
         swiglu = a.workload == "gpt-swiglu"
+        docs = a.workload == "gpt-1.3b-docs"
         ov = common + [f"Global.local_batch_size={local}", f"Global.micro_batch_size={local}", f"Distributed.dp_degree={world}",
                        "Distributed.mp_degree=1", "Distributed.pp_degree=1", "Distributed.sharding.sharding_degree=1"]
         if a.layers:
             ov.append(f"Model.num_layers={a.layers}")
-        recipe = "pretrain_gpt_1.3B_swiglu_single_card.yaml" if swiglu else "pretrain_gpt_1.3B_single_card.yaml"
+        recipe = ("pretrain_gpt_1.3B_swiglu_single_card.yaml" if swiglu else
+                  "pretrain_gpt_1.3B_packed_docs_single_card.yaml" if docs else "pretrain_gpt_1.3B_single_card.yaml")
         cfg = C.get_config(os.path.join(CFG, "nlp/gpt", recipe), ov, nranks=world)
         seq = 1024
         cfg.Data.Train["dataset"] = C.AttrDict(name="SyntheticGPTDataset", max_seq_len=seq, vocab_size=cfg.Model.vocab_size)
@@ -77,10 +81,18 @@ def main():
         h = cfg.Model.hidden_size
         ffn = cfg.Model.get("ffn_hidden_size") or (swiglu_ffn_size(h) if swiglu else 4 * h)
         name = f"GPT 1.3B ({'SwiGLU' if swiglu else 'GELU'} FFN, F = {ffn}), dp{world}, {local} x {seq} tokens/GPU, recompute {cfg.Model.get('use_recompute')}"
+        if docs:
+            from paddlefleetx_b200.data.dataset.gpt_dataset import SyntheticGPTDataset
+
+            name += ", packed documents of 128-383 tokens, reset_attention_mask"
+            doc_set = SyntheticGPTDataset(max_seq_len=seq, vocab_size=cfg.Model.vocab_size, reset_position_ids=True, document_length=256)
 
         def make_batch(g):
             t = torch.randint(0, cfg.Model.vocab_size, (local, seq + 1), generator=g)
-            pos = torch.arange(seq).unsqueeze(0).expand(local, seq).contiguous()
+            if docs:
+                pos = torch.stack([torch.from_numpy(doc_set[int(torch.randint(0, 1 << 20, (1,), generator=g))][1]) for _ in range(local)])
+            else:
+                pos = torch.arange(seq).unsqueeze(0).expand(local, seq).contiguous()
             return [t[:, :-1].contiguous(), pos, t[:, 1:].contiguous(), torch.ones(local, seq)]
     elif a.workload == "moe":
         local = a.local_batch or 8
