@@ -174,10 +174,11 @@ class MultiHeadAttention(nn.Module):
 
         hcg = getattr(_env, "_hcg", None)           # only an already-built topology counts (get_hcg() would build a default one)
         if hcg is not None and getattr(hcg, "cp", 1) > 1:
-            if self.group > 1:
-                raise ValueError("num_key_value_heads < num_attention_heads is not supported with context parallelism (Distributed.cp_degree > 1)")
-            self.cp_group = hcg.get_context_parallel_group()
             self.cp_mode = getattr(hcg, "cp_mode", "ulysses")
+            if self.group > 1 and self.cp_mode != "ring":
+                raise ValueError("num_key_value_heads < num_attention_heads is not supported with Ulysses context parallelism "
+                                 "(Distributed.cp_degree > 1); use Distributed.cp_mode: ring")
+            self.cp_group = hcg.get_context_parallel_group()
             assert self.cp_mode == "ring" or self.local_heads % self.cp_group.nranks == 0, \
                 f"local heads {self.local_heads} % cp {self.cp_group.nranks} (Ulysses shards heads; cp_mode: ring has no such limit)"
 
@@ -250,15 +251,16 @@ class MultiHeadAttention(nn.Module):
                 positions = local_positions(q.shape[1], self.cp_group.nranks, self.cp_group.rank, self.cp_mode, q.device).expand(q.shape[0], -1)
             q, k = OF.rope(q.contiguous(), positions), OF.rope(k.contiguous(), positions)      # ``positions`` are global (sliced with the tokens)
         if self.cp_mode == "ring":
-            assert attn_mask is None, "ring attention builds the causal mask from the zigzag layout; explicit masks are not sharded"
-            from ....parallel.ring_attention import ring_attention
+            from ....parallel.ring_attention import RingDocumentMask, ring_attention
 
+            assert attn_mask is None or isinstance(attn_mask, RingDocumentMask), \
+                "ring attention builds the causal mask from the zigzag layout; explicit masks are not sharded"
             p = self.attn_dropout if self.training else 0.0
             if p > 0:
                 with get_rng_state_tracker().rng_state("local_seed"):
-                    out = ring_attention(q, k, v, self.cp_group, True, p, self.head_dim ** -0.5)
+                    out = ring_attention(q, k, v, self.cp_group, True, p, self.head_dim ** -0.5, doc=attn_mask)
             else:
-                out = ring_attention(q, k, v, self.cp_group, True, 0.0, self.head_dim ** -0.5)
+                out = ring_attention(q, k, v, self.cp_group, True, 0.0, self.head_dim ** -0.5, doc=attn_mask)
             return self._project_out(out)
         q, k, v = (C.seq_head_all_to_all(t, self.cp_group, 2, 1) for t in (q, k, v))           # [b, s, H/c, d]
         out = recompute(self._core, q, k, v, attn_mask) if (self.recompute_core and self.training) else self._core(q, k, v, attn_mask)
@@ -514,8 +516,15 @@ class GPTModel(nn.Module):
             past = caches[0].length
             position_ids = torch.arange(past, past + input_ids.shape[1], device=input_ids.device).unsqueeze(0).expand_as(input_ids)
         if self.reset_attention_mask and attention_mask is None and position_ids is not None and caches is None:
-            # one mask for every layer: on CUDA one launch derives the per-row key bounds and their per-tile min / max
-            attention_mask = ATT.DocumentMask.from_positions(position_ids)
+            # one mask for every layer: on CUDA one launch derives the per-row key bounds and their per-tile min / max (under ring context
+            # parallelism those of every block this rank meets on the ring, from its zigzag shard of the position ids)
+            attn = self.decoder.layers[0].self_attn
+            if attn.cp_group is not None and attn.cp_mode == "ring":
+                from ....parallel.ring_attention import RingDocumentMask
+
+                attention_mask = RingDocumentMask.from_positions(position_ids, attn.cp_group.nranks, attn.cp_group.rank)
+            else:
+                attention_mask = ATT.DocumentMask.from_positions(position_ids)
         x = self.embeddings(input_ids, position_ids)
         x = self.decoder(x, attention_mask, caches, position_ids)
         if self.sequence_parallel:

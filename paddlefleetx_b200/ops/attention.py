@@ -69,12 +69,17 @@ class DocumentMask:
             return cls(ks, tmin, tmax)
         i = torch.arange(s, dtype=torch.int64, device=src.device)
         ks = (i - src) if from_positions else src
-        ks = torch.minimum(ks.clamp_min(0), i).to(torch.int32)
+        return cls.with_tile_bounds(torch.minimum(ks.clamp_min(0), i).to(torch.int32))
+
+    @classmethod
+    def with_tile_bounds(cls, key_start: torch.Tensor) -> "DocumentMask":
+        """The mask of int32 ``key_start`` ``[b, sq]`` taken as it is, with its per-tile minimum / maximum computed in PyTorch."""
+        b, s = key_start.shape
         t = -(-s // cls.TILE)
         pad = t * cls.TILE - s
-        lo = torch.nn.functional.pad(ks, (0, pad), value=torch.iinfo(torch.int32).max).view(b, t, cls.TILE).amin(-1)
-        hi = torch.nn.functional.pad(ks, (0, pad), value=0).view(b, t, cls.TILE).amax(-1)
-        return cls(ks, lo, hi)
+        lo = torch.nn.functional.pad(key_start, (0, pad), value=torch.iinfo(torch.int32).max).view(b, t, cls.TILE).amin(-1)
+        hi = torch.nn.functional.pad(key_start, (0, pad), value=0).view(b, t, cls.TILE).amax(-1)
+        return cls(key_start, lo, hi)
 
     @classmethod
     def from_positions(cls, position_ids: torch.Tensor) -> "DocumentMask":
@@ -114,7 +119,7 @@ def _native_ok(q, k, v, attn_mask, causal, needs_grad: bool, doc: Optional[Docum
     d = q.shape[-1]
     if d not in (64, 128) or q.shape[1] < 1 or (causal and k.shape[1] < q.shape[1]):
         return False
-    if doc is not None and (not causal or k.shape[1] != q.shape[1] or doc.shape != (q.shape[0], q.shape[1]) or not doc.key_start.is_cuda):
+    if doc is not None and ((causal and k.shape[1] != q.shape[1]) or doc.shape != (q.shape[0], q.shape[1]) or not doc.key_start.is_cuda):
         return False
     if k.dim() != 4 or v.shape != k.shape or _q_heads(q) % k.shape[2] or (q.dim() == 5 and q.shape[2] != k.shape[2]):
         return False
@@ -181,7 +186,7 @@ class _FlashAttnFn(torch.autograd.Function):
         if packed is not None:
             q, k, v = _split_packed(packed)
         if doc is not None:
-            out, lse = _native.require().attention_fwd_doc(q, k, v, *doc.bounds(), float(scale), float(dropout_p), int(seed))
+            out, lse = _native.require().attention_fwd_doc(q, k, v, *doc.bounds(), float(scale), float(dropout_p), int(seed), bool(causal))
         else:
             out, lse = _native.require().attention_fwd_v2(q, k, v, bool(causal), float(scale), float(dropout_p), int(seed))
         OF._count()
@@ -208,7 +213,7 @@ class _FlashAttnFn(torch.autograd.Function):
             dq, dk, dv = torch.empty_like(q, memory_format=torch.contiguous_format), torch.empty_like(k, memory_format=torch.contiguous_format), \
                 torch.empty_like(v, memory_format=torch.contiguous_format)
         if ctx.doc is not None:
-            _native.require().attention_bwd_doc(q, k, v, out, dout, lse, dq, dk, dv, *ctx.doc.bounds(), scale, dropout_p, seed)
+            _native.require().attention_bwd_doc(q, k, v, out, dout, lse, dq, dk, dv, *ctx.doc.bounds(), scale, dropout_p, seed, causal)
         else:
             _native.require().attention_bwd(q, k, v, out, dout, lse, dq, dk, dv, causal, scale, dropout_p, seed)
         OF._count(4)           # memset is a driver call; prep + main + dq convert (+ the tensor-core kernel counted once more for its size)

@@ -87,9 +87,11 @@ __device__ __forceinline__ void tma_tile(const CUtensorMap* m, bool swapped, uin
 // so the multi-head kernels are compiled exactly as without it).  The CTA then owns a key tile of one (batch, K/V head) and walks the
 // query tiles of all G heads of the group in turn, with each head's lse / delta, dropout key, Q column and dQ column, while dK / dV
 // stay in registers: they are exact sums written once, with no atomics, and deterministic.
-// kDoc (causal, Sq == Sk): query i attends keys [doc.key_start[b, i], i].  A query tile whose tile_min lies past the key tile's last key
-// holds no pair of it: the producer does not load it and the consumers do not wait for it (both skip by the same rule, for every head of
-// a group).  The ring slots count only the tiles that run.  key_start need not be monotone: the rule uses the tile's minimum.
+// kDoc: query i attends keys [doc.key_start[b, i], i] when causal (Sq == Sk), or [doc.key_start[b, i], Sk) otherwise (any Sq, Sk).  A
+// query tile whose tile_min lies past the key tile's last key holds no pair of it: the producer does not load it and the consumers do not
+// wait for it (both skip by the same rule, for every head of a group).  The ring slots count only the tiles that run.  key_start need not
+// be monotone: the rule uses the tile's minimum.  Without the causal diagonal a key tile may be reached by no query tile at all: it then
+// waits only for its own K / V and writes dK = dV = 0.
 template <int kHd, bool kBf16, bool kGqa, bool kDoc = false>
 __global__ void __launch_bounds__(kBwThreads, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v,
@@ -192,7 +194,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
       const int q0 = iter_q0(it);
       const DocBounds cur = nxt;
       if constexpr (kDoc) nxt = doc_bounds(it + 1);
-      if (kDoc && cur.lo > k0 + kKv - 1) continue;   // never the diagonal tile i_begin (its tile_min <= its first query = k0)
+      if (kDoc && cur.lo > k0 + kKv - 1) continue;   // causal: never the diagonal tile i_begin (its tile_min <= its first query = k0)
       const int slot = kDoc ? n_run++ : it;
       const int st = slot % S::kStages;
       const int hq = iter_head(it);
@@ -445,14 +447,15 @@ cudaError_t attention_bwd(const AttnView& q, const AttnView& k, const AttnView& 
 }
 
 cudaError_t attention_bwd_doc(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, const AttnView& dout, const float* lse,
-                              const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int S,
-                              int H, int Hkv, int D, float scale, AttnDropout drop, const AttnDocMask& doc, int dtype, cudaStream_t st) {
-  if ((D != 64 && D != 128) || (dtype != 0 && dtype != 1) || B < 1 || S < 1) return cudaErrorInvalidValue;
+                              const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int Sq,
+                              int Sk, int H, int Hkv, int D, float scale, bool causal, AttnDropout drop, const AttnDocMask& doc, int dtype,
+                              cudaStream_t st) {
+  if ((D != 64 && D != 128) || (dtype != 0 && dtype != 1) || B < 1 || Sq < 1 || Sk < 1 || (causal && Sk != Sq)) return cudaErrorInvalidValue;
   if (H < 1 || Hkv < 1 || H % Hkv != 0 || (Hkv < H && (q.sg % 8 || dq.sg % 8))) return cudaErrorInvalidValue;
   if (doc.key_start == nullptr || doc.tile_min == nullptr || doc.tile_max == nullptr) return cudaErrorInvalidValue;
   for (const AttnView* t : {&q, &k, &v, &out, &dout, &dq, &dk, &dv}) if (!view_ok(*t)) return cudaErrorInvalidValue;
 #define PFX_BWD(HD, BF, GQA) \
-  attention_bwd_impl<HD, BF, GQA, true>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, S, S, H, Hkv, scale, true, drop, st, doc)
+  attention_bwd_impl<HD, BF, GQA, true>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, Sq, Sk, H, Hkv, scale, causal, drop, st, doc)
   if (Hkv < H) {
     if (dtype == 1) return D == 128 ? PFX_BWD(128, true, true) : PFX_BWD(64, true, true);
     return D == 128 ? PFX_BWD(128, false, true) : PFX_BWD(64, false, true);

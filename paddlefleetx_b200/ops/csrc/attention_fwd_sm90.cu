@@ -57,16 +57,16 @@ __device__ __forceinline__ void tma3(const CUtensorMap* m, bool swapped, uint32_
 // the multi-head kernels are compiled exactly as without it); query head h loads Q at column (h / G) * gs_q + (h % G) * hs_q and K / V
 // of head h / G.  The work order keeps the heads of one batch adjacent, so the G query heads of a group stream the same K / V tiles
 // at about the same time and share them through L2.
-// kDoc (with kCausal, Sq == Sk): query i attends keys [doc.key_start[b, i], i] (AttnDocMask).  A 64-query tile starts at key tile
-// tile_min / 128 in the producer and the consumers alike, and only tiles with key0 < tile_max (plus the diagonal / ragged ones) pay
-// per-element compares.
+// kDoc: query i attends keys [doc.key_start[b, i], i] with kCausal (Sq == Sk), or [doc.key_start[b, i], Sk) without it (the off-diagonal
+// blocks of ring attention, any Sq and Sk; key_start = Sk leaves the row empty).  A 64-query tile starts at key tile tile_min / 128 in the
+// producer and the consumers alike, and only tiles with key0 < tile_max (plus the diagonal / ragged ones) pay per-element compares.  A
+// non-causal tile with tile_min >= Sk loads no K / V at all; its rows keep l = 0, which the epilogue writes as out = 0, lse = -inf.
 template <int kD, bool kCausal, bool kBf16, bool kGqa, bool kDoc = false>
 __global__ void __launch_bounds__(kFaThreads, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v,
                      uint16_t* __restrict__ out, int64_t o_sb, int64_t o_ss, int64_t o_sh, float* __restrict__ lse, int B, int Sq, int Sk, int H,
                      float scale_log2, int hs_q, int hs_k, int hs_v, uint32_t swapped, uint32_t drop_thresh16, float inv_keep, uint64_t seed,
                      int G, int gs_q, AttnDocMask doc) {
-  static_assert(!kDoc || kCausal, "the document mask is a causal mask with a per-row lower key bound");
   using S = FaSmem<kD>;
   constexpr int kPanels = kD / 64;                 // 64-element (128-byte) column panels of a D-wide tile
   extern __shared__ uint8_t smem_raw[];
@@ -89,7 +89,12 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
     return kCausal ? min(n_kv_all, (q_tile * kFaQ + kFaQ - 1 + (Sk - Sq)) / kFaKv + 1) : n_kv_all;
   };
   auto tile_j0 = [&](int q_tile, int b) {            // first key tile a query tile attends to
-    return kDoc ? __ldg(doc.tile_min + (size_t)b * n_q_tiles + q_tile) / kFaKv : 0;
+    if constexpr (kDoc) {
+      const int lo = __ldg(doc.tile_min + (size_t)b * n_q_tiles + q_tile);
+      return (!kCausal && lo >= Sk) ? n_kv_all : lo / kFaKv;
+    } else {
+      return 0;
+    }
   };
 
   if (warp == 4 && elect_one()) {
@@ -290,10 +295,12 @@ cudaError_t launch_fa_dt(const AttnView& q, const AttnView& k, const AttnView& v
 }
 
 template <bool kBf16, bool kGqa>
-cudaError_t launch_fa_doc(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int S, int H, int Hkv, int D,
-                          float scale, AttnDropout drop, const AttnDocMask& doc, cudaStream_t st) {
-  if (D == 128) return launch_fa<128, true, kBf16, kGqa, true>(q, k, v, out, lse, B, S, S, H, Hkv, scale, drop, st, doc);
-  return launch_fa<64, true, kBf16, kGqa, true>(q, k, v, out, lse, B, S, S, H, Hkv, scale, drop, st, doc);
+cudaError_t launch_fa_doc(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H,
+                          int Hkv, int D, float scale, bool causal, AttnDropout drop, const AttnDocMask& doc, cudaStream_t st) {
+  if (D == 128) return causal ? launch_fa<128, true, kBf16, kGqa, true>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, scale, drop, st, doc)
+                              : launch_fa<128, false, kBf16, kGqa, true>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, scale, drop, st, doc);
+  return causal ? launch_fa<64, true, kBf16, kGqa, true>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, scale, drop, st, doc)
+                : launch_fa<64, false, kBf16, kGqa, true>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, scale, drop, st, doc);
 }
 
 }  // namespace
@@ -311,18 +318,18 @@ cudaError_t attention_fwd_v2(const AttnView& q, const AttnView& k, const AttnVie
                     : launch_fa_dt<false, false>(q, k, v, out, lse, B, Sq, Sk, H, H, D, scale, causal, drop, st);
 }
 
-cudaError_t attention_fwd_doc(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int S, int H, int Hkv,
-                              int D, float scale, AttnDropout drop, const AttnDocMask& doc, int dtype, cudaStream_t st) {
-  if ((D != 64 && D != 128) || (dtype != 0 && dtype != 1) || B < 1 || S < 1) return cudaErrorInvalidValue;
+cudaError_t attention_fwd_doc(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H,
+                              int Hkv, int D, float scale, bool causal, AttnDropout drop, const AttnDocMask& doc, int dtype, cudaStream_t st) {
+  if ((D != 64 && D != 128) || (dtype != 0 && dtype != 1) || B < 1 || Sq < 1 || Sk < 1 || (causal && Sk != Sq)) return cudaErrorInvalidValue;
   if (H < 1 || Hkv < 1 || H % Hkv != 0 || (Hkv < H && q.sg % 8)) return cudaErrorInvalidValue;
   if (doc.key_start == nullptr || doc.tile_min == nullptr || doc.tile_max == nullptr) return cudaErrorInvalidValue;
   for (const AttnView* t : {&q, &k, &v, &out})
     if (t->ptr == nullptr || (reinterpret_cast<uintptr_t>(t->ptr) % 16) || t->sb % 8 || t->ss % 8 || t->sh % 8) return cudaErrorInvalidValue;
   if (Hkv < H)
-    return dtype == 1 ? launch_fa_doc<true, true>(q, k, v, out, lse, B, S, H, Hkv, D, scale, drop, doc, st)
-                      : launch_fa_doc<false, true>(q, k, v, out, lse, B, S, H, Hkv, D, scale, drop, doc, st);
-  return dtype == 1 ? launch_fa_doc<true, false>(q, k, v, out, lse, B, S, H, H, D, scale, drop, doc, st)
-                    : launch_fa_doc<false, false>(q, k, v, out, lse, B, S, H, H, D, scale, drop, doc, st);
+    return dtype == 1 ? launch_fa_doc<true, true>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, D, scale, causal, drop, doc, st)
+                      : launch_fa_doc<false, true>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, D, scale, causal, drop, doc, st);
+  return dtype == 1 ? launch_fa_doc<true, false>(q, k, v, out, lse, B, Sq, Sk, H, H, D, scale, causal, drop, doc, st)
+                    : launch_fa_doc<false, false>(q, k, v, out, lse, B, Sq, Sk, H, H, D, scale, causal, drop, doc, st);
 }
 
 // ---- document-mask bounds: key_start[b, i] = clamp(i - pos[b, i], 0, i) (or clamp(src, 0, i) when src already holds key starts), and
@@ -356,6 +363,56 @@ cudaError_t attention_doc_bounds(const int64_t* src, bool from_positions, int B,
   if (src == nullptr || B < 1 || S < 1 || B > 65535) return cudaErrorInvalidValue;
   const int n_tiles = (S + 63) / 64;
   attn_doc_bounds_kernel<<<dim3(n_tiles, B), 64, 0, st>>>(src, from_positions ? 1 : 0, S, n_tiles, key_start, tile_min, tile_max);
+  return cudaGetLastError();
+}
+
+// ---- ring attention's document blocks: one 64-thread block per (64-row tile, b, src) writes the block's key_start (the number of the
+// block's keys that lie before the row's document) and the tile's minimum / maximum.  Local row i sits at global position r h + i (i < h)
+// or (2c - 1 - r) h + i - h; its document starts at clamp(g - pos, 0, g).
+__global__ void attn_ring_doc_bounds_kernel(const int64_t* __restrict__ pos, int s_l, int c, int r, int* __restrict__ out) {
+  __shared__ int red[2][2];
+  const int src = blockIdx.z, b = blockIdx.y, B = gridDim.y, h = s_l / 2;
+  const int rows = src > r ? h : s_l, n_tiles = (rows + 63) / 64;
+  if ((int)blockIdx.x >= n_tiles) return;                         // uniform over the block
+  size_t off = 0;                                                 // this block's arrays follow those of every smaller src
+  for (int j = 0; j < src; ++j) {
+    const int rj = j > r ? h : s_l;
+    off += (size_t)B * (rj + 2 * ((rj + 63) / 64));
+  }
+  int* key_start = out + off;
+  int* tile_min = key_start + (size_t)B * rows;
+  int* tile_max = tile_min + (size_t)B * n_tiles;
+  const int i = blockIdx.x * 64 + threadIdx.x;
+  int lo = INT_MAX, hi = 0;
+  if (i < rows) {
+    const int lr = src > r ? h + i : i;                            // src > r: the block holds the second local chunk only
+    const int64_t g = lr < h ? (int64_t)r * h + lr : (int64_t)(2 * c - 1 - r) * h + (lr - h);
+    int64_t ks_g = g - pos[(size_t)b * s_l + lr];
+    ks_g = ks_g < 0 ? 0 : (ks_g > g ? g : ks_g);
+    const int64_t a0 = (int64_t)src * h;                          // the block's key chunks: [a0, a0 + h) and, unless src < r, [b0, b0 + h)
+    const int64_t b0 = (int64_t)(2 * c - 1 - src) * h;
+    auto below = [&](int64_t start) { const int64_t n = ks_g - start; return (int)(n < 0 ? 0 : (n > h ? h : n)); };
+    const int v = below(a0) + (src >= r ? below(b0) : 0);
+    key_start[(size_t)b * rows + i] = v;
+    lo = hi = v;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    lo = min(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+    hi = max(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+  }
+  if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = lo; red[1][threadIdx.x >> 5] = hi; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    tile_min[(size_t)b * n_tiles + blockIdx.x] = min(red[0][0], red[0][1]);
+    tile_max[(size_t)b * n_tiles + blockIdx.x] = max(red[1][0], red[1][1]);
+  }
+}
+
+cudaError_t attention_ring_doc_bounds(const int64_t* pos, int B, int s_l, int c, int r, int* out, cudaStream_t st) {
+  if (pos == nullptr || out == nullptr || B < 1 || B > 65535 || s_l < 2 || s_l % 2 || c < 1 || c > 65535 || r < 0 || r >= c)
+    return cudaErrorInvalidValue;
+  attn_ring_doc_bounds_kernel<<<dim3((s_l + 63) / 64, B, c), 64, 0, st>>>(pos, s_l, c, r, out);
   return cudaGetLastError();
 }
 

@@ -897,29 +897,59 @@ std::vector<at::Tensor> attention_doc_bounds(const at::Tensor& src, bool from_po
   return {ks, tmin, tmax};
 }
 
+// Ring attention's document blocks (see pfx::attention_ring_doc_bounds) from this rank's zigzag-local position ids int64 [B, s_l]: returns,
+// for src = 0 .. c - 1 in turn, (key_start [B, rows], tile_min, tile_max [B, ceil(rows / 64)]) with rows = s_l (src <= r) or s_l / 2
+// (src > r), all views of one int32 buffer written by one kernel.
+std::vector<at::Tensor> attention_ring_doc_bounds(const at::Tensor& pos, int64_t c, int64_t r) {
+  TORCH_CHECK(pos.is_cuda() && pos.dim() == 2 && pos.is_contiguous() && pos.scalar_type() == at::kLong, "attention_ring_doc_bounds: int64 [B, s_l] CUDA tensor");
+  TORCH_CHECK(pos.size(0) >= 1 && pos.size(0) <= 65535 && pos.size(1) >= 2 && pos.size(1) % 2 == 0, "attention_ring_doc_bounds: 1 <= B <= 65535, even s_l");
+  TORCH_CHECK(c >= 1 && c <= 65535 && r >= 0 && r < c, "attention_ring_doc_bounds: 0 <= r < c");
+  const c10::cuda::CUDAGuard guard(pos.device());
+  const int64_t B = pos.size(0), S = pos.size(1);
+  int64_t total = 0;
+  for (int64_t j = 0; j < c; ++j) {
+    const int64_t rows = j > r ? S / 2 : S;
+    total += B * (rows + 2 * ((rows + 63) / 64));
+  }
+  auto buf = at::empty({total}, pos.options().dtype(at::kInt));
+  PFX_CUDA_CHECK(pfx::attention_ring_doc_bounds(pos.data_ptr<int64_t>(), (int)B, (int)S, (int)c, (int)r, buf.data_ptr<int>(), cur_stream()));
+  std::vector<at::Tensor> views;
+  int64_t off = 0;
+  for (int64_t j = 0; j < c; ++j) {
+    const int64_t rows = j > r ? S / 2 : S, T = (rows + 63) / 64;
+    views.push_back(buf.narrow(0, off, B * rows).view({B, rows}));
+    views.push_back(buf.narrow(0, off + B * rows, B * T).view({B, T}));
+    views.push_back(buf.narrow(0, off + B * (rows + T), B * T).view({B, T}));
+    off += B * (rows + 2 * T);
+  }
+  return views;
+}
+
 static pfx::AttnDocMask attn_doc(const at::Tensor& ks, const at::Tensor& tmin, const at::Tensor& tmax, int64_t B, int64_t S, const char* fn) {
   const int64_t T = (S + 63) / 64;
   for (const at::Tensor* t : {&ks, &tmin, &tmax})
     TORCH_CHECK(t->is_cuda() && t->is_contiguous() && t->scalar_type() == at::kInt, fn, ": document bounds must be contiguous int32 CUDA tensors");
-  TORCH_CHECK(ks.numel() == B * S && tmin.numel() == B * T && tmax.numel() == B * T, fn, ": document bounds must be [B, S] and [B, ceil(S / 64)]");
+  TORCH_CHECK(ks.numel() == B * S && tmin.numel() == B * T && tmax.numel() == B * T, fn, ": document bounds must be [B, Sq] and [B, ceil(Sq / 64)]");
   return pfx::AttnDocMask{ks.data_ptr<int>(), tmin.data_ptr<int>(), tmax.data_ptr<int>()};
 }
 
-// Causal flash attention under a document mask (self-attention, Sq == Sk): query i attends keys [key_start[b, i], i].  The bounds come
-// from attention_doc_bounds.  Views as in attention_fwd_v2.
+// Flash attention under a document mask.  causal (self-attention, Sq == Sk): query i attends keys [key_start[b, i], i]; otherwise keys
+// [key_start[b, i], Sk) for any Sq and Sk (key_start = Sk: an empty row, out = 0 and lse = -inf).  The bounds come from
+// attention_doc_bounds or attention_ring_doc_bounds.  Views as in attention_fwd_v2.
 std::vector<at::Tensor> attention_fwd_doc(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v, const at::Tensor& key_start,
-                                          const at::Tensor& tile_min, const at::Tensor& tile_max, double scale, double dropout_p, int64_t seed) {
+                                          const at::Tensor& tile_min, const at::Tensor& tile_max, double scale, double dropout_p, int64_t seed,
+                                          bool causal) {
   const int64_t Hkv = attn_kv_heads(q, k, "attention_fwd_doc");
   const int64_t H = attn_q_heads(q), D = q.size(q.dim() - 1);
-  TORCH_CHECK(k.sizes() == v.sizes() && q.size(0) == k.size(0) && q.size(1) == k.size(1) && D == k.size(3),
-              "attention_fwd_doc: shape mismatch (self-attention: q and k have one sequence length)");
+  TORCH_CHECK(k.sizes() == v.sizes() && q.size(0) == k.size(0) && (!causal || q.size(1) == k.size(1)) && D == k.size(3),
+              "attention_fwd_doc: shape mismatch (causal self-attention: q and k have one sequence length)");
   TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type(), "attention_fwd_doc: q, k, v must have one dtype");
   const pfx::AttnDocMask doc = attn_doc(key_start, tile_min, tile_max, q.size(0), q.size(1), "attention_fwd_doc");
   const c10::cuda::CUDAGuard guard(q.device());
   auto out = at::empty({q.size(0), q.size(1), H, D}, q.options());
   auto lse = at::empty({q.size(0), H, q.size(1)}, q.options().dtype(at::kFloat));
   PFX_CUDA_CHECK(pfx::attention_fwd_doc(attn_qview(q, "q", Hkv), attn_view(k, "k"), attn_view(v, "v"), attn_view(out, "out"), lse.data_ptr<float>(),
-                                        (int)q.size(0), (int)q.size(1), (int)H, (int)Hkv, (int)D, (float)scale,
+                                        (int)q.size(0), (int)q.size(1), (int)k.size(1), (int)H, (int)Hkv, (int)D, (float)scale, causal,
                                         pfx::AttnDropout{(float)dropout_p, (uint64_t)seed}, doc, dtype_code(q), cur_stream()));
   return {out, lse};
 }
@@ -927,29 +957,30 @@ std::vector<at::Tensor> attention_fwd_doc(const at::Tensor& q, const at::Tensor&
 // Backward of attention_fwd_doc: writes dq / dk / dv into the given (possibly strided) views.
 void attention_bwd_doc(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v, const at::Tensor& out, const at::Tensor& dout, const at::Tensor& lse,
                        at::Tensor& dq, at::Tensor& dk, at::Tensor& dv, const at::Tensor& key_start, const at::Tensor& tile_min, const at::Tensor& tile_max,
-                       double scale, double dropout_p, int64_t seed) {
+                       double scale, double dropout_p, int64_t seed, bool causal) {
   const int64_t Hkv = attn_kv_heads(q, k, "attention_bwd_doc");
   const int64_t H = attn_q_heads(q), D = q.size(q.dim() - 1);
   TORCH_CHECK(D == 128 || D == 64, "attention_bwd_doc: head_dim must be 64 or 128");
-  TORCH_CHECK(k.sizes() == v.sizes() && q.size(0) == k.size(0) && q.size(1) == k.size(1) && D == k.size(3), "attention_bwd_doc: k / v shape mismatch");
+  TORCH_CHECK(k.sizes() == v.sizes() && q.size(0) == k.size(0) && (!causal || q.size(1) == k.size(1)) && D == k.size(3),
+              "attention_bwd_doc: k / v shape mismatch");
   TORCH_CHECK(k.sizes() == dk.sizes() && k.sizes() == dv.sizes(), "attention_bwd_doc: dk / dv must have the shape of k");
   TORCH_CHECK(q.sizes() == dq.sizes(), "attention_bwd_doc: dq must have the shape of q");
   const std::vector<int64_t> o_shape{q.size(0), q.size(1), H, D};
-  TORCH_CHECK(out.sizes() == at::IntArrayRef(o_shape) && dout.sizes() == at::IntArrayRef(o_shape), "attention_bwd_doc: out / dout must be [B,S,H,D]");
+  TORCH_CHECK(out.sizes() == at::IntArrayRef(o_shape) && dout.sizes() == at::IntArrayRef(o_shape), "attention_bwd_doc: out / dout must be [B,Sq,H,D]");
   TORCH_CHECK(lse.is_cuda() && lse.is_contiguous() && lse.scalar_type() == at::kFloat && lse.numel() == q.size(0) * q.size(1) * H, "attention_bwd_doc: lse");
   for (const at::Tensor* t : std::initializer_list<const at::Tensor*>{&k, &v, &out, &dout, &dq, &dk, &dv})
     TORCH_CHECK(t->scalar_type() == q.scalar_type(), "attention_bwd_doc: q, k, v, out, dout and the gradients must have one dtype");
   const pfx::AttnDocMask doc = attn_doc(key_start, tile_min, tile_max, q.size(0), q.size(1), "attention_bwd_doc");
   const c10::cuda::CUDAGuard guard(q.device());
-  const int64_t B = q.size(0), S = q.size(1);
-  const int64_t s_pad = (S + 63) / 64 * 64;
+  const int64_t B = q.size(0), Sq = q.size(1), Sk = k.size(1);
+  const int64_t s_pad = (Sq + 63) / 64 * 64;
   auto f32 = q.options().dtype(at::kFloat);
-  auto dq_acc = at::empty({B, S, H, D}, f32);
+  auto dq_acc = at::empty({B, Sq, H, D}, f32);
   auto stats = at::empty({2, B * H * s_pad}, f32);
   PFX_CUDA_CHECK(pfx::attention_bwd_doc(attn_qview(q, "q", Hkv), attn_view(k, "k"), attn_view(v, "v"), attn_view(out, "out"), attn_view(dout, "dout"),
                                         lse.data_ptr<float>(), attn_qview(dq, "dq", Hkv), attn_view(dk, "dk"), attn_view(dv, "dv"), dq_acc.data_ptr<float>(),
-                                        stats[0].data_ptr<float>(), stats[1].data_ptr<float>(), (int)B, (int)S, (int)H, (int)Hkv, (int)D, (float)scale,
-                                        pfx::AttnDropout{(float)dropout_p, (uint64_t)seed}, doc, dtype_code(q), cur_stream()));
+                                        stats[0].data_ptr<float>(), stats[1].data_ptr<float>(), (int)B, (int)Sq, (int)Sk, (int)H, (int)Hkv, (int)D,
+                                        (float)scale, causal, pfx::AttnDropout{(float)dropout_p, (uint64_t)seed}, doc, dtype_code(q), cur_stream()));
 }
 
 at::Tensor attention_decode_packed(const at::Tensor& qkv, at::Tensor& k, at::Tensor& v, c10::optional<at::Tensor> mask, const at::Tensor& write_idx,
@@ -1207,8 +1238,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("attention_fwd_v2", &attention_fwd_v2);
   m.def("attention_bwd", &attention_bwd);
   m.def("attention_doc_bounds", &attention_doc_bounds);
-  m.def("attention_fwd_doc", &attention_fwd_doc);
-  m.def("attention_bwd_doc", &attention_bwd_doc);
+  m.def("attention_ring_doc_bounds", &attention_ring_doc_bounds);
+  m.def("attention_fwd_doc", &attention_fwd_doc, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("key_start"), py::arg("tile_min"),
+        py::arg("tile_max"), py::arg("scale"), py::arg("dropout_p"), py::arg("seed"), py::arg("causal") = true);
+  m.def("attention_bwd_doc", &attention_bwd_doc, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("out"), py::arg("dout"), py::arg("lse"),
+        py::arg("dq"), py::arg("dk"), py::arg("dv"), py::arg("key_start"), py::arg("tile_min"), py::arg("tile_max"), py::arg("scale"),
+        py::arg("dropout_p"), py::arg("seed"), py::arg("causal") = true);
   m.def("attention_decode", &attention_decode);
   m.def("attention_decode_packed", &attention_decode_packed);
   m.def("gemm_bias_gelu_dual", &gemm_bias_gelu_dual);

@@ -29,12 +29,13 @@ struct AttnDropout {
 cudaError_t attention_fwd_v2(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H,
                              int Hkv, int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st);
 
-// Intra-document causal mask for packed sequences (self-attention, Sq == Sk == S): query i of batch row b attends the keys
-// [key_start[b, i], i], with 0 <= key_start[b, i] <= i.  tile_min / tile_max hold the minimum / maximum of key_start over each
-// 64-query tile ([B, ceil(S / 64)]); the kernels skip whole key tiles from them and compare per element only on boundary tiles.
+// Intra-document mask for packed sequences: query i of batch row b attends the keys [key_start[b, i], i] when causal (self-attention,
+// Sq == Sk, 0 <= key_start[b, i] <= i), or [key_start[b, i], Sk) when not (0 <= key_start[b, i] <= Sk; Sk leaves the row empty: out = 0,
+// lse = -inf).  tile_min / tile_max hold the minimum / maximum of key_start over each 64-query tile ([B, ceil(Sq / 64)]); the kernels
+// skip whole key tiles from them and compare per element only on boundary tiles.
 struct AttnDocMask {
-  const int* key_start;     // int32 [B, S]
-  const int* tile_min;      // int32 [B, ceil(S / 64)]
+  const int* key_start;     // int32 [B, Sq]
+  const int* tile_min;      // int32 [B, ceil(Sq / 64)]
   const int* tile_max;
 };
 
@@ -42,9 +43,15 @@ struct AttnDocMask {
 // clamp(src[b, i], 0, i) otherwise, and the per-tile bounds of AttnDocMask.  src int64 [B, S].
 cudaError_t attention_doc_bounds(const int64_t* src, bool from_positions, int B, int S, int* key_start, int* tile_min, int* tile_max, cudaStream_t st);
 
-// attention_fwd_v2 with causal = true under a document mask (separate kernel instantiations).
-cudaError_t attention_fwd_doc(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int S, int H, int Hkv,
-                              int D, float scale, AttnDropout drop, const AttnDocMask& doc, int dtype, cudaStream_t st);
+// Ring attention's document blocks: for every source rank src of a ring of c (this rank r), the block's key_start in its own key coordinates
+// and tile bounds, from this rank's zigzag-local position ids pos int64 [B, s_l] (s_l = 2h: global chunks r and 2c - 1 - r).  The blocks
+// are src == r: all rows x both own chunks (causal); src < r: all rows x chunk src; src > r: rows [h, 2h) x chunks src and 2c - 1 - src.
+// out holds, per src in turn, key_start [B, rows], tile_min [B, ceil(rows / 64)], tile_max [B, ceil(rows / 64)] (rows = s_l or h).
+cudaError_t attention_ring_doc_bounds(const int64_t* pos, int B, int s_l, int c, int r, int* out, cudaStream_t st);
+
+// attention_fwd_v2 under a document mask (separate kernel instantiations): causal with Sq == Sk, or non-causal with any Sq, Sk.
+cudaError_t attention_fwd_doc(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H,
+                              int Hkv, int D, float scale, bool causal, AttnDropout drop, const AttnDocMask& doc, int dtype, cudaStream_t st);
 
 // Backward.  Workspace: dq_acc fp32 [B, Sq, H, D] (zeroed by the call), lse2 / delta fp32 [B, H, round_up(Sq, 64)].
 // dq / dk / dv may be strided views (e.g. slices of one packed [B, S, H, 3, D] gradient buffer).  D is 64 or 128; dtype as above.
@@ -53,10 +60,12 @@ cudaError_t attention_bwd(const AttnView& q, const AttnView& k, const AttnView& 
                           const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int Sq,
                           int Sk, int H, int Hkv, int D, float scale, bool causal, AttnDropout drop, int dtype, cudaStream_t st);
 
-// attention_bwd with causal = true under a document mask: a key tile skips every query tile whose tile_min lies past its last key.
+// attention_bwd under a document mask (causal with Sq == Sk, or non-causal): a key tile skips every query tile whose tile_min lies past its
+// last key; a key tile that no query reaches writes dk = dv = 0.
 cudaError_t attention_bwd_doc(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, const AttnView& dout, const float* lse,
-                              const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int S,
-                              int H, int Hkv, int D, float scale, AttnDropout drop, const AttnDocMask& doc, int dtype, cudaStream_t st);
+                              const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int Sq,
+                              int Sk, int H, int Hkv, int D, float scale, bool causal, AttnDropout drop, const AttnDocMask& doc, int dtype,
+                              cudaStream_t st);
 
 // Evoformer gated attention (head width 32, H even): softmax(scale QK^T + mask_bias[g, k] + pair_bias[g / groups_per_pair, h, q, k]) V * sigmoid(gate).
 // q / out / gate [G, Sq, H, 32], k / v [G, Sk, H, 32] bf16 contiguous; mask_bias fp32 [G, Sk]; pair_bias bf16; stats fp32 [2, G, H, Sq]: the

@@ -17,6 +17,10 @@ def check_device(device: str):
         raise ValueError(f"unsupported device '{device}': this framework targets NVIDIA H100 (gpu) with a cpu functional path")
 
 
+def _cp_mode(d) -> str:
+    return str(d.get("cp_mode", "ulysses") or "ulysses").lower()
+
+
 def check_kv_heads(m, d, compress) -> None:
     """``Model.num_key_value_heads`` (grouped-query attention; unset = ``num_attention_heads``)."""
     heads, kv = m.get("num_attention_heads"), m.get("num_key_value_heads")
@@ -28,8 +32,9 @@ def check_kv_heads(m, d, compress) -> None:
         raise ValueError(f"num_key_value_heads ({kv}) must be divisible by mp_degree ({d.mp_degree}): tensor parallelism shards whole K/V groups")
     if kv == heads:
         return
-    if d.get("cp_degree", 1) > 1:
-        raise ValueError("num_key_value_heads < num_attention_heads is not supported with context parallelism (Distributed.cp_degree > 1)")
+    if d.get("cp_degree", 1) > 1 and _cp_mode(d) != "ring":
+        raise ValueError("num_key_value_heads < num_attention_heads is not supported with Ulysses context parallelism (Distributed.cp_degree > 1): "
+                         "use Distributed.cp_mode: ring")
     prune = compress.get("Prune") or {}
     if prune.get("enable", False) and prune.get("prune_heads", True):
         raise ValueError("Compress.Prune head pruning does not support num_key_value_heads < num_attention_heads; "
@@ -56,7 +61,8 @@ def check_ffn_activation(m, d, compress) -> None:
 
 def check_document_mask(m, d, data) -> None:
     """``Model.reset_attention_mask`` (attention stays inside each packed document) needs ``Data.*.dataset.reset_position_ids``, which
-    produces the position ids the mask is derived from, and a layout whose attention sees whole sequences with their positions."""
+    produces the position ids the mask is derived from, and a layout whose attention sees its shard's positions: no pipeline, and context
+    parallelism in ring mode only (each rank derives its blocks' masks from its zigzag shard of the position ids)."""
     if not m.get("reset_attention_mask", False):
         return
     sets = [data[k].get("dataset", {}) or {} for k in ("Train", "Eval") if data.get(k)]
@@ -66,9 +72,14 @@ def check_document_mask(m, d, data) -> None:
     if d.get("pp_degree", 1) > 1:
         raise ValueError("Model.reset_attention_mask is not supported with pipeline parallelism (Distributed.pp_degree > 1): "
                          "later stages receive no position ids")
-    if d.get("cp_degree", 1) > 1:
-        raise ValueError("Model.reset_attention_mask is not supported with context parallelism (Distributed.cp_degree > 1): "
-                         "the ring and Ulysses layouts shard the sequence")
+    if d.get("cp_degree", 1) > 1 and _cp_mode(d) != "ring":
+        raise ValueError("Model.reset_attention_mask is not supported with Ulysses context parallelism (Distributed.cp_degree > 1): "
+                         "use Distributed.cp_mode: ring")
+    c = d.get("cp_degree", 1) or 1
+    for ds in sets:
+        if c > 1 and ds.get("max_seq_len") and ds["max_seq_len"] % (2 * c):
+            raise ValueError(f"Model.reset_attention_mask with cp_mode: ring needs max_seq_len ({ds['max_seq_len']}) to be a multiple of "
+                             f"2 x cp_degree = {2 * c} (two zigzag chunks per rank)")
 
 
 def check_config(cfg):
