@@ -7,7 +7,8 @@ gather before the MLM head, ``ignore_index = -1`` criterion, sequence-classifica
 
 Beyond the reference (needed for BASELINE config #3, ERNIE-10B mp4 + ZeRO-3): the MLM decoder is vocabulary-parallel
 and the loss uses the vocab-parallel CE kernel (the reference leaves both replicated — SURVEY §2.7); attention runs the
-fused flash path with a padding mask.
+fused flash path with a padding mask: ``ErnieModel.forward`` builds one ``KeyPaddingMask`` per forward pass from the 2-D mask or the
+pad tokens, and every layer hands it to the key-padding flash kernels (the explicit-mask paths add its ``[b, 1, 1, s]`` form).
 """
 from __future__ import annotations
 
@@ -114,6 +115,8 @@ class ErnieSelfAttention(nn.Module):
         return (z, z.clone())
 
     def forward(self, x, attn_mask=None):
+        """``attn_mask``: a ``KeyPaddingMask`` (the flash kernels read it as it is, also on the gathered ``[s, b, ...]`` views of sequence
+        parallelism) or an additive tensor."""
         if self.sequence_parallel:
             # x: [s/n, b, h] -> one all-gather (backward: reduce-scatter) -> [s, b, h]; the column-parallel GEMMs then run on the gathered
             # tensor directly (no identity/all-reduce pair: the gather's backward already sums the partial input gradients)
@@ -127,7 +130,7 @@ class ErnieSelfAttention(nn.Module):
         p = self.attn_dropout if self.training else 0.0
         scale = self.head_dim ** -0.5
         if self.use_flash_attn:
-            m = None if attn_mask is None else attn_mask.to(q.dtype)
+            m = attn_mask if attn_mask is None or isinstance(attn_mask, ATT.KeyPaddingMask) else attn_mask.to(q.dtype)
             if p > 0:
                 with get_rng_state_tracker().rng_state("local_seed"):
                     o = ATT.attention(q, k, v, causal=False, dropout_p=p, scale=scale, attn_mask=m)
@@ -293,7 +296,12 @@ class ErnieModel(nn.Module):
                              else "You have to specify either input_ids or inputs_embeds")
         dtype = self.pooler.dense.weight.dtype
         past_len = past_key_values[0][0].shape[2] if past_key_values is not None else None
-        if attention_mask is None:
+        detailed = past_key_values is not None or bool(use_cache) or output_hidden_states or output_attentions or return_dict
+        if not detailed and attention_mask is None and input_ids is not None:
+            attention_mask = ATT.KeyPaddingMask.from_ids(input_ids, self.pad_token_id, dtype)
+        elif not detailed and attention_mask is not None and attention_mask.dim() == 2:
+            attention_mask = ATT.KeyPaddingMask.from_valid(attention_mask, dtype)
+        elif attention_mask is None:
             if input_ids is not None:
                 pad = (input_ids == self.pad_token_id)
                 attention_mask = pad[:, None, None, :].to(dtype) * -1e4
@@ -302,7 +310,6 @@ class ErnieModel(nn.Module):
         elif attention_mask.dim() == 2:
             attention_mask = (1.0 - attention_mask[:, None, None, :].to(dtype)) * -1e4
         x = self.embeddings(input_ids, token_type_ids, position_ids, task_type_ids, inputs_embeds, past_len)
-        detailed = past_key_values is not None or bool(use_cache) or output_hidden_states or output_attentions or return_dict
         if not detailed:
             if self.sequence_parallel:
                 assert x.shape[1] % C.group_size(self.mp_group) == 0, "sequence length must divide by the tensor-parallel degree under sequence parallelism"

@@ -13,6 +13,9 @@ dtype):
   * packed documents (``DocumentMask``: query ``i`` attends keys ``[key_start[b, i], i]``): the same kernels, in separate
     instantiations that skip the key tiles outside a query tile's documents; other head sizes, fp32 and CPU tensors run the dense
     boolean form of the mask through SDPA,
+  * bidirectional key padding (``KeyPaddingMask``: every query of row ``b`` attends the valid keys of row ``b``, as ERNIE's padding mask):
+    separate non-causal multi-head instantiations that never load the key tiles past the last valid key; grouped K/V heads, other head
+    sizes, fp32 and CPU tensors run the mask's additive ``[b, 1, 1, s]`` form through SDPA,
   * explicit masks, other head sizes, mixed dtypes, fp32 and CPU tensors: PyTorch SDPA — a *library* call, reported as such by the launch
     accounting (it does not count towards ``gpu_launches``); ``PFX_NATIVE_ATTN=0`` forces it everywhere,
   * the unfused reference path (QK^T -> fused causal softmax -> PV) used when ``use_flash_attn=False`` — this mirrors reference
@@ -111,7 +114,91 @@ class DocumentMask:
         return self.key_start, self.tile_min, self.tile_max
 
 
-def _native_ok(q, k, v, attn_mask, causal, needs_grad: bool, doc: Optional[DocumentMask] = None) -> bool:
+class KeyPaddingMask:
+    """Bidirectional attention over the valid keys of each batch row: every query of row ``b`` attends key ``j`` iff ``valid[b, j]``.  A
+    row without any valid key attends every key, which is what the additive ``-1e4`` mask gives (one constant added to every logit of a
+    row leaves its softmax unchanged).  Any pattern is exact; the native kernels read
+
+      * ``key_bits`` int32 ``[b, ceil(s / 32)]``: the validity bits, 32 keys per word (bit ``j % 32`` of word ``j // 32``),
+      * ``key_end`` int32 ``[b]``: 1 + the last valid key; key tiles at or past it are never loaded,
+      * ``key_dense`` int32 ``[b]``: the first invalid key; key tiles entirely below it need no per-element compare.
+
+    Build it once per forward pass (``from_valid`` / ``from_ids``) and hand the same object to every layer: on CUDA the derivation is
+    one native launch.  ``additive()`` gives the ``[b, 1, 1, s]`` tensor that the explicit-mask paths (SDPA, ``core_attention``) add to
+    the logits, built by the same formula as ERNIE's padding mask, in ``dtype``."""
+
+    WORD = 32
+    _NATIVE_DTYPES = (torch.bool, torch.uint8, torch.int32, torch.int64, torch.float32, torch.float16, torch.bfloat16)   # read by the bounds kernel
+
+    def __init__(self, key_bits: torch.Tensor, key_end: torch.Tensor, key_dense: torch.Tensor, src: torch.Tensor, from_ids: bool,
+                 pad_id: int, dtype: torch.dtype):
+        self.key_bits, self.key_end, self.key_dense = key_bits, key_end, key_dense
+        self._src, self._from_ids, self._pad_id, self.dtype = src, from_ids, pad_id, dtype
+
+    @classmethod
+    def _build(cls, src: torch.Tensor, from_ids: bool, pad_id: int, dtype) -> "KeyPaddingMask":
+        if src.dim() != 2 or src.shape[0] < 1 or src.shape[1] < 1:
+            raise ValueError(f"KeyPaddingMask expects a [batch, seq] tensor, got shape {tuple(src.shape)}")
+        if from_ids and src.dtype not in (torch.int32, torch.int64):
+            raise ValueError(f"KeyPaddingMask.from_ids expects int32 / int64 ids, got {src.dtype}")
+        if src.is_cuda:
+            from . import _native
+            from . import functional as OF
+
+            native = src if from_ids or src.dtype in cls._NATIVE_DTYPES else src != 0
+            bits, end, dense = _native.require().attention_key_pad_bounds(native.contiguous(), bool(from_ids), int(pad_id))
+            OF._count()
+            return cls(bits, end, dense, src, from_ids, pad_id, dtype)
+        valid = (src != pad_id) if from_ids else (src != 0)
+        b, s = valid.shape
+        i = torch.arange(s, device=src.device)
+        last = torch.where(valid, i, -1).amax(-1)
+        first_bad = torch.where(valid, s, i).amin(-1)
+        empty = last < 0
+        valid = valid | empty.unsqueeze(-1)
+        end = torch.where(empty, s, last + 1).to(torch.int32)
+        dense = torch.where(empty, s, first_bad).to(torch.int32)
+        w = -(-s // cls.WORD)
+        padded = torch.nn.functional.pad(valid, (0, w * cls.WORD - s)).view(b, w, cls.WORD).to(torch.int64)
+        words = (padded << torch.arange(cls.WORD, device=src.device)).sum(-1)
+        bits = torch.where(words >= 1 << 31, words - (1 << 32), words).to(torch.int32)      # the uint32 words, stored as int32
+        return cls(bits, end, dense, src, from_ids, pad_id, dtype)
+
+    @classmethod
+    def from_valid(cls, mask: torch.Tensor, dtype=torch.float32) -> "KeyPaddingMask":
+        """``[b, s]`` validity (bool, integers or 0 / 1 floats; nonzero = a real token).  ``additive()`` is ``(1 - mask) * -1e4``."""
+        return cls._build(mask, False, 0, dtype)
+
+    @classmethod
+    def from_ids(cls, input_ids: torch.Tensor, pad_id: int, dtype=torch.float32) -> "KeyPaddingMask":
+        """``[b, s]`` token ids; keys equal to ``pad_id`` are padding.  ``additive()`` is ``(input_ids == pad_id) * -1e4``."""
+        return cls._build(input_ids, True, int(pad_id), dtype)
+
+    @property
+    def shape(self):
+        return tuple(self._src.shape)
+
+    def dense(self) -> torch.Tensor:
+        """bool ``[b, 1, 1, s]``, True where a key is attended (every key of a row without valid keys)."""
+        s = self._src.shape[1]
+        j = torch.arange(s, device=self.key_bits.device)
+        words = self.key_bits.to(torch.int64)[:, j // self.WORD]
+        return ((words >> (j % self.WORD)) & 1).bool()[:, None, None, :]
+
+    def additive(self, dtype=None) -> torch.Tensor:
+        """The ``[b, 1, 1, s]`` additive mask (0 for valid keys, -1e4 for padding) in ``dtype`` (default: the dtype the mask was built
+        for), bit for bit the tensor ERNIE has always added to its logits."""
+        dtype = self.dtype if dtype is None else dtype
+        if self._from_ids:
+            return (self._src == self._pad_id)[:, None, None, :].to(dtype) * -1e4
+        return (1.0 - self._src[:, None, None, :].to(dtype)) * -1e4
+
+    def bounds(self):
+        return self.key_bits, self.key_end, self.key_dense
+
+
+def _native_ok(q, k, v, attn_mask, causal, needs_grad: bool, doc: Optional[DocumentMask] = None,
+               pad: Optional[KeyPaddingMask] = None) -> bool:
     from .functional import tensor_core_dtype
 
     if not _NATIVE or attn_mask is not None or not q.is_cuda or not tensor_core_dtype(q, k, v):
@@ -120,6 +207,9 @@ def _native_ok(q, k, v, attn_mask, causal, needs_grad: bool, doc: Optional[Docum
     if d not in (64, 128) or q.shape[1] < 1 or (causal and k.shape[1] < q.shape[1]):
         return False
     if doc is not None and ((causal and k.shape[1] != q.shape[1]) or doc.shape != (q.shape[0], q.shape[1]) or not doc.key_start.is_cuda):
+        return False
+    if pad is not None and (causal or q.dim() != 4 or k.shape[2] != q.shape[2] or pad.shape != (k.shape[0], k.shape[1])
+                            or not pad.key_bits.is_cuda):
         return False
     if k.dim() != 4 or v.shape != k.shape or _q_heads(q) % k.shape[2] or (q.dim() == 5 and q.shape[2] != k.shape[2]):
         return False
@@ -185,14 +275,16 @@ class _FlashAttnFn(torch.autograd.Function):
 
         if packed is not None:
             q, k, v = _split_packed(packed)
-        if doc is not None:
+        if isinstance(doc, KeyPaddingMask):
+            out, lse = _native.require().attention_fwd_keypad(q, k, v, *doc.bounds(), float(scale), float(dropout_p), int(seed))
+        elif doc is not None:
             out, lse = _native.require().attention_fwd_doc(q, k, v, *doc.bounds(), float(scale), float(dropout_p), int(seed), bool(causal))
         else:
             out, lse = _native.require().attention_fwd_v2(q, k, v, bool(causal), float(scale), float(dropout_p), int(seed))
         OF._count()
         ctx.save_for_backward(q, k, v, out, lse)
         ctx.cfg = (packed is not None, bool(causal), float(scale), float(dropout_p), int(seed))
-        ctx.doc = doc            # the tile bounds of the forward serve the backward
+        ctx.doc = doc            # the tile (or key-padding) bounds of the forward serve the backward
         return out
 
     @staticmethod
@@ -212,7 +304,9 @@ class _FlashAttnFn(torch.autograd.Function):
         else:
             dq, dk, dv = torch.empty_like(q, memory_format=torch.contiguous_format), torch.empty_like(k, memory_format=torch.contiguous_format), \
                 torch.empty_like(v, memory_format=torch.contiguous_format)
-        if ctx.doc is not None:
+        if isinstance(ctx.doc, KeyPaddingMask):
+            _native.require().attention_bwd_keypad(q, k, v, out, dout, lse, dq, dk, dv, *ctx.doc.bounds(), scale, dropout_p, seed)
+        elif ctx.doc is not None:
             _native.require().attention_bwd_doc(q, k, v, out, dout, lse, dq, dk, dv, *ctx.doc.bounds(), scale, dropout_p, seed, causal)
         else:
             _native.require().attention_bwd(q, k, v, out, dout, lse, dq, dk, dv, causal, scale, dropout_p, seed)
@@ -240,18 +334,23 @@ def flash_attention_packed(mix: torch.Tensor, causal: bool = True, dropout_p: fl
 
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = True, dropout_p: float = 0.0,
               scale: Optional[float] = None, attn_mask=None) -> torch.Tensor:
-    """``attn_mask``: a boolean / additive tensor (SDPA), or a ``DocumentMask`` (the native kernels where they apply; ``causal`` is
-    implied)."""
+    """``attn_mask``: a boolean / additive tensor (SDPA), a ``DocumentMask`` (the native kernels where they apply; ``causal`` is
+    implied) or a ``KeyPaddingMask`` (likewise; non-causal is implied)."""
     needs_grad = torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad)
     doc = attn_mask if isinstance(attn_mask, DocumentMask) else None
+    pad = attn_mask if isinstance(attn_mask, KeyPaddingMask) else None
     if doc is not None:
         causal, attn_mask = True, None
-    if _native_ok(q, k, v, attn_mask, causal, needs_grad, doc):
+    if pad is not None:
+        causal, attn_mask = False, None
+    if _native_ok(q, k, v, attn_mask, causal, needs_grad, doc, pad):
         sc = float(scale if scale is not None else q.shape[-1] ** -0.5)
         seed = _dropout_seed(dropout_p, q.shape[0] * q.shape[2] * q.shape[1] * k.shape[1])
-        return _FlashAttnFn.apply(None, q, k, v, causal, sc, dropout_p, seed, doc)
+        return _FlashAttnFn.apply(None, q, k, v, causal, sc, dropout_p, seed, doc if pad is None else pad)
     if doc is not None:
         attn_mask = doc.dense()
+    if pad is not None:
+        attn_mask = pad.additive().to(q.dtype)
     qt, kt, vt = (t.transpose(1, 2) for t in (q, k, v))           # [b, h, s, d]
     if attn_mask is not None:
         causal = False
@@ -269,7 +368,7 @@ def core_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: flo
     if k.shape[2] != q.shape[2]:
         g = q.shape[2] // k.shape[2]
         k, v = k.repeat_interleave(g, dim=2), v.repeat_interleave(g, dim=2)
-    if isinstance(attn_mask, DocumentMask):
+    if isinstance(attn_mask, (DocumentMask, KeyPaddingMask)):
         attn_mask = attn_mask.additive()
     qt, kt, vt = (t.transpose(1, 2) for t in (q, k, v))
     scores = torch.matmul(qt, kt.transpose(-1, -2))

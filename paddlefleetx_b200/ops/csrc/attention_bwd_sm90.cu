@@ -76,7 +76,10 @@ struct BwParams {
   float inv_keep;
   uint64_t seed;
   int G, gs_q;                         // grouped-query instantiation only: query heads per K/V head, q stride between groups
-  AttnDocMask doc;                     // document-mask instantiation only
+  union {
+    AttnDocMask doc;                   // document-mask instantiation only
+    AttnKeyPad pad;                    // key-padding instantiation only
+  };
 };
 
 __device__ __forceinline__ void tma_tile(const CUtensorMap* m, bool swapped, uint32_t bar, uint32_t dst, int col, int s, int b) {
@@ -92,11 +95,15 @@ __device__ __forceinline__ void tma_tile(const CUtensorMap* m, bool swapped, uin
 // wait for it (both skip by the same rule, for every head of a group).  The ring slots count only the tiles that run.  key_start need not
 // be monotone: the rule uses the tile's minimum.  Without the causal diagonal a key tile may be reached by no query tile at all: it then
 // waits only for its own K / V and writes dK = dV = 0.
-template <int kHd, bool kBf16, bool kGqa, bool kDoc = false>
+// kKeyPad (non-causal, MHA): a key tile with k0 >= key_end[b] loads nothing, waits on no barrier and writes dK = dV = 0.  The thread's two
+// key rows keep their validity bits for the whole query loop; tiles that reach past key_dense[b] zero P^T (and with it dS^T) on invalid
+// rows, so dQ gets nothing from padded keys.
+template <int kHd, bool kBf16, bool kGqa, bool kDoc = false, bool kKeyPad = false>
 __global__ void __launch_bounds__(kBwThreads, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v,
                      const __grid_constant__ CUtensorMap tmap_do, const __grid_constant__ CUtensorMap tmap_dq, const __grid_constant__ BwParams prm) {
   using S = BwSmem<kHd>;
+  static_assert(!kKeyPad || (!kGqa && !kDoc), "key padding: multi-head attention only");
   constexpr int kPanels = S::kPanels;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -123,7 +130,9 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
   const int n_q_tiles = (prm.Sq + kQt - 1) / kQt;
   const int i_begin = prm.causal ? max(0, k0 - off) / kQt : 0;
   const int n_head_iter = n_q_tiles - i_begin;    // >= 1 for every key tile that holds a valid key
-  const int n_iter = kGqa ? n_head_iter * prm.G : n_head_iter;
+  // kKeyPad: a key tile at or past key_end runs no iteration
+  const bool pad_dead = kKeyPad && k0 >= __ldg(prm.pad.key_end + b);
+  const int n_iter = pad_dead ? 0 : kGqa ? n_head_iter * prm.G : n_head_iter;
   // iteration it -> (query head, first query): the query tiles of the group's first head, then the next head's, ...
   auto iter_head = [&](int it) { return kGqa ? h * prm.G + it / n_head_iter : h; };
   auto iter_q0 = [&](int it) { return (i_begin + (kGqa ? it % n_head_iter : it)) * kQt; };
@@ -145,7 +154,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
 
   if (warp == 4) {
     // ==== TMA producer
-    if (elect_one()) {
+    if (elect_one() && !pad_dead) {
       mbar_arrive_expect_tx(kv_full, 2 * S::kKBytes);
       for (int p = 0; p < kPanels; ++p) {
         tma_tile(&tmap_k, prm.swapped & 2u, kv_full, s_k + p * 8192, h * prm.hs_k + p * 64, k0, b);
@@ -187,7 +196,18 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
     float dv[kHd / 2], dk[kHd / 2];
 #pragma unroll
     for (int i = 0; i < kHd / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
-    mbar_wait(kv_full, 0);
+    bool kvalid[2] = {true, true};                                    // kKeyPad: the validity bits of this thread's key rows
+    int pad_dense = 0;
+    if constexpr (kKeyPad) {
+      pad_dense = __ldg(prm.pad.key_dense + b);
+      const int n_words = (prm.Sk + 31) / 32;
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int kg = k0 + k_row + 8 * hh;
+        kvalid[hh] = kg < prm.Sk && ((__ldg(prm.pad.key_bits + (size_t)b * n_words + kg / 32) >> (kg % 32)) & 1u);
+      }
+    }
+    if (!pad_dead) mbar_wait(kv_full, 0);
     int n_run = 0;
     DocBounds nxt = doc_bounds(0);
     for (int it = 0; it < n_iter; ++it) {
@@ -219,7 +239,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
       const float* dl_s = lse_s + kQt;
       // masks are decided per tile (warp-uniform branches): only diagonal / ragged tiles pay per-element compares
       const bool tile_mask = (prm.causal && (k0 + kKv - 1 > q0 + off)) || (k0 + kKv > prm.Sk) ||
-                             (kDoc && k0 < cur.hi);
+                             (kDoc && k0 < cur.hi) || (kKeyPad && k0 + kKv > pad_dense);
       uint32_t pw[kQt / 4], dsw[kQt / 4];                             // P_drop^T and dS^T as packed 16-bit pairs, in wgmma A-fragment order
 #pragma unroll
       for (int g = 0; g < kQt / 8; ++g) {
@@ -238,6 +258,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
               if (q0 + qc < prm.Sq && kg < __ldg(ks + q0 + qc)) p0 = 0.f;
               if (q0 + qc + 1 < prm.Sq && kg < __ldg(ks + q0 + qc + 1)) p1 = 0.f;
             }
+            if (kKeyPad && !kvalid[hh]) { p0 = 0.f; p1 = 0.f; }
           }
           float d0 = dp[4 * g + 2 * hh], d1 = dp[4 * g + 2 * hh + 1];
           float pd0 = p0 * p_to_pdrop, pd1 = p1 * p_to_pdrop;
@@ -379,11 +400,11 @@ bool make_map(CUtensorMap* m, const AttnView& t, int dtype, int B, int S, int H,
 
 }  // namespace
 
-template <int kHd, bool kBf16, bool kGqa, bool kDoc = false>
+template <int kHd, bool kBf16, bool kGqa, bool kDoc = false, bool kKeyPad = false>
 static cudaError_t attention_bwd_impl(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, const AttnView& dout, const float* lse,
                                       const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int Sq,
                                       int Sk, int H, int Hkv, float scale, bool causal, AttnDropout drop, cudaStream_t st,
-                                      const AttnDocMask& doc = AttnDocMask{}) {
+                                      const AttnDocMask& doc = AttnDocMask{}, const AttnKeyPad& pad = AttnKeyPad{}) {
   const int G = H / Hkv;
   constexpr int D = kHd;
   constexpr int dt = kBf16 ? 1 : 0;
@@ -417,14 +438,14 @@ static cudaError_t attention_bwd_impl(const AttnView& q, const AttnView& k, cons
   prm.drop_thresh16 = drop.p > 0.f ? (uint32_t)(drop.p * 65536.f + 0.5f) : 0u;
   prm.inv_keep = drop.p > 0.f ? 1.f / (1.f - drop.p) : 1.f;
   prm.seed = drop.seed;
-  prm.doc = doc;
+  if (kKeyPad) prm.pad = pad; else prm.doc = doc;
   static bool attr_set = false;
   if (!attr_set) {
-    if ((e = cudaFuncSetAttribute(attention_bwd_kernel<kHd, kBf16, kGqa, kDoc>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal)) != cudaSuccess) return e;
+    if ((e = cudaFuncSetAttribute(attention_bwd_kernel<kHd, kBf16, kGqa, kDoc, kKeyPad>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal)) != cudaSuccess) return e;
     attr_set = true;
   }
   const int n_kv = (Sk + kKv - 1) / kKv;
-  attention_bwd_kernel<kHd, kBf16, kGqa, kDoc><<<(unsigned)(n_kv * B * Hkv), kBwThreads, S::kTotal, st>>>(tq, tk, tv, tdo, tdq, prm);
+  attention_bwd_kernel<kHd, kBf16, kGqa, kDoc, kKeyPad><<<(unsigned)(n_kv * B * Hkv), kBwThreads, S::kTotal, st>>>(tq, tk, tv, tdo, tdq, prm);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   attn_bwd_dq_convert_kernel<kBf16, kGqa><<<1184, 256, 0, st>>>(dq_acc, (uint16_t*)const_cast<void*>(dq.ptr), dq.sb, dq.ss, dq.sh, B, Sq, H, kHd, G, dq.sg);
   return cudaGetLastError();
@@ -462,6 +483,20 @@ cudaError_t attention_bwd_doc(const AttnView& q, const AttnView& k, const AttnVi
   }
   if (dtype == 1) return D == 128 ? PFX_BWD(128, true, false) : PFX_BWD(64, true, false);
   return D == 128 ? PFX_BWD(128, false, false) : PFX_BWD(64, false, false);
+#undef PFX_BWD
+}
+
+cudaError_t attention_bwd_keypad(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, const AttnView& dout, const float* lse,
+                                 const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int Sq,
+                                 int Sk, int H, int D, float scale, AttnDropout drop, const AttnKeyPad& pad, int dtype, cudaStream_t st) {
+  if ((D != 64 && D != 128) || (dtype != 0 && dtype != 1) || B < 1 || Sq < 1 || Sk < 1 || H < 1) return cudaErrorInvalidValue;
+  if (pad.key_bits == nullptr || pad.key_end == nullptr || pad.key_dense == nullptr) return cudaErrorInvalidValue;
+  for (const AttnView* t : {&q, &k, &v, &out, &dout, &dq, &dk, &dv}) if (!view_ok(*t)) return cudaErrorInvalidValue;
+#define PFX_BWD(HD, BF) \
+  attention_bwd_impl<HD, BF, false, false, true>(q, k, v, out, dout, lse, dq, dk, dv, dq_acc, lse2, delta, B, Sq, Sk, H, H, scale, false, drop, st, \
+                                                 AttnDocMask{}, pad)
+  if (dtype == 1) return D == 128 ? PFX_BWD(128, true) : PFX_BWD(64, true);
+  return D == 128 ? PFX_BWD(128, false) : PFX_BWD(64, false);
 #undef PFX_BWD
 }
 

@@ -19,6 +19,7 @@
 // (FlashAttention-2 library on Ampere mma.sync).
 #include <climits>
 #include <cstdio>
+#include <type_traits>
 
 #include "pfx_ptx.cuh"
 #include "pfx_gemm.h"
@@ -61,12 +62,18 @@ __device__ __forceinline__ void tma3(const CUtensorMap* m, bool swapped, uint32_
 // blocks of ring attention, any Sq and Sk; key_start = Sk leaves the row empty).  A 64-query tile starts at key tile tile_min / 128 in the
 // producer and the consumers alike, and only tiles with key0 < tile_max (plus the diagonal / ragged ones) pay per-element compares.  A
 // non-causal tile with tile_min >= Sk loads no K / V at all; its rows keep l = 0, which the epilogue writes as out = 0, lse = -inf.
-template <int kD, bool kCausal, bool kBf16, bool kGqa, bool kDoc = false>
+// kKeyPad (non-causal, MHA; `doc` is then an AttnKeyPad): the producer and the consumers walk the key tiles [0, ceil(key_end[b] / 128)),
+// and only tiles that reach past key_dense[b] compare per element.  A compare tile's 128 bits are four words that every thread of the
+// warpgroup reads with __ldg, issued before the S product so that their latency hides behind it: all 128 threads read the same 16
+// bytes (one broadcast transaction per warp, L1-resident for the heads of a row), while staging them through the producer would add
+// shared memory and barrier traffic to every tile for the one tile per right-padded row that needs them.
+template <int kD, bool kCausal, bool kBf16, bool kGqa, bool kDoc = false, bool kKeyPad = false>
 __global__ void __launch_bounds__(kFaThreads, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v,
                      uint16_t* __restrict__ out, int64_t o_sb, int64_t o_ss, int64_t o_sh, float* __restrict__ lse, int B, int Sq, int Sk, int H,
                      float scale_log2, int hs_q, int hs_k, int hs_v, uint32_t swapped, uint32_t drop_thresh16, float inv_keep, uint64_t seed,
-                     int G, int gs_q, AttnDocMask doc) {
+                     int G, int gs_q, std::conditional_t<kKeyPad, AttnKeyPad, AttnDocMask> doc) {
+  static_assert(!kKeyPad || (!kCausal && !kGqa && !kDoc), "key padding: non-causal multi-head attention only");
   using S = FaSmem<kD>;
   constexpr int kPanels = kD / 64;                 // 64-element (128-byte) column panels of a D-wide tile
   extern __shared__ uint8_t smem_raw[];
@@ -85,8 +92,9 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
   const int n_items = n_q_tiles * hb_count;
   // item w -> (query tile, h, b): all (h, b) of the longest tile first, then the next shorter one, ...
   auto item_tile = [&](int w) { return n_q_tiles - 1 - w / hb_count; };
-  auto tile_n_kv = [&](int q_tile) {                 // key tiles a query tile attends to
-    return kCausal ? min(n_kv_all, (q_tile * kFaQ + kFaQ - 1 + (Sk - Sq)) / kFaKv + 1) : n_kv_all;
+  auto tile_n_kv = [&](int q_tile, int b) {          // key tiles a query tile attends to
+    if constexpr (kKeyPad) return (__ldg(doc.key_end + b) + kFaKv - 1) / kFaKv;
+    else return kCausal ? min(n_kv_all, (q_tile * kFaQ + kFaQ - 1 + (Sk - Sq)) / kFaKv + 1) : n_kv_all;
   };
   auto tile_j0 = [&](int q_tile, int b) {            // first key tile a query tile attends to
     if constexpr (kDoc) {
@@ -112,7 +120,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
       int it = 0;
       for (int w = blockIdx.x; w < n_items; w += gridDim.x, ++it) {
         const int q_tile = item_tile(w), hb = w % hb_count, h = hb % H, b = hb / H;
-        const int n_kv = tile_n_kv(q_tile);
+        const int n_kv = tile_n_kv(q_tile, b);
         const int q_col = kGqa ? (h / G) * gs_q + (h % G) * hs_q : h * hs_q;
         const int hk = kGqa ? h / G : h;
         mbar_wait(q_empty, ((uint32_t)it & 1u) ^ 1u);
@@ -141,7 +149,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
     int it = 0;
     for (int w = blockIdx.x; w < n_items; w += gridDim.x, ++it) {
       const int q_tile = item_tile(w), hb = w % hb_count, h = hb % H, b = hb / H;
-      const int n_kv = tile_n_kv(q_tile);
+      const int n_kv = tile_n_kv(q_tile, b);
       const int q0 = q_tile * kFaQ;
       float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // per row (row_lo, row_lo + 8): running maximum (log2 units), this thread's part of the row sum
       float o[kD / 2];
@@ -158,11 +166,21 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
           doc_ks[hh] = row_g < Sq ? __ldg(doc.key_start + (size_t)b * Sq + row_g) : 0;
         }
       }
+      int pad_dense = 0;                              // kKeyPad: the first invalid key of row b
+      if constexpr (kKeyPad) pad_dense = __ldg(doc.key_dense + b);
       mbar_wait(q_full, (uint32_t)it & 1u);
       for (int j = tile_j0(q_tile, b); j < n_kv; ++j, ++t) {
         const int stage = t & 1;
         const uint32_t sk = smem_kv + stage * S::kStageBytes, sv = sk + S::kKBytes;
         mbar_wait(kv_full(stage), (t >> 1) & 1u);
+        uint32_t kbits[kFaKv / 32];                // kKeyPad compare tiles: the tile's bit words, shifted to this thread's column pair
+        if constexpr (kKeyPad) {
+          const bool cmp = j * kFaKv + kFaKv > pad_dense;
+          const int w0 = j * (kFaKv / 32), n_words = (Sk + 31) / 32;
+#pragma unroll
+          for (int w = 0; w < kFaKv / 32; ++w)
+            kbits[w] = !cmp ? ~0u : (w0 + w < n_words ? __ldg(doc.key_bits + (size_t)b * n_words + w0 + w) : 0u) >> col_in8;
+        }
         float s[kFaKv / 2];                        // s[4 g + e]: row row_lo + 8 (e / 2), key 8 g + col_in8 + (e % 2)
         wgmma_fence();
 #pragma unroll
@@ -173,13 +191,16 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
         wgmma_commit();
         wgmma_wait<0>();
         const int key0 = j * kFaKv;
-        const bool need_mask = (kCausal && key0 + kFaKv - 1 > q0 + (Sk - Sq)) || (key0 + kFaKv > Sk) || (kDoc && key0 < doc_max);
+        const bool need_mask = (kCausal && key0 + kFaKv - 1 > q0 + (Sk - Sq)) || (key0 + kFaKv > Sk) || (kDoc && key0 < doc_max) ||
+                               (kKeyPad && key0 + kFaKv > pad_dense);
         if (need_mask) {
 #pragma unroll
           for (int i = 0; i < kFaKv / 2; ++i) {
             const int cg = key0 + 8 * (i >> 2) + col_in8 + (i & 1);
             const int row_g = q0 + row_lo + 8 * ((i >> 1) & 1);
             if (cg >= Sk || (kCausal && cg > row_g + (Sk - Sq)) || (kDoc && cg < doc_ks[(i >> 1) & 1])) s[i] = -INFINITY;
+            if constexpr (kKeyPad)                    // column 8 g + col_in8 + e of the tile: word g / 4, bit 8 (g % 4) + col_in8 + e
+              if (!((kbits[i >> 4] >> (8 * ((i >> 2) & 3) + (i & 1))) & 1u)) s[i] = -INFINITY;
           }
         }
         float f[2], m_use[2];
@@ -248,9 +269,9 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
   }
 }
 
-template <int kD, bool kCausal, bool kBf16, bool kGqa, bool kDoc = false>
+template <int kD, bool kCausal, bool kBf16, bool kGqa, bool kDoc = false, bool kKeyPad = false>
 cudaError_t launch_fa(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H, int Hkv,
-                      float scale, AttnDropout drop, cudaStream_t st, AttnDocMask doc = AttnDocMask{}) {
+                      float scale, AttnDropout drop, cudaStream_t st, std::conditional_t<kKeyPad, AttnKeyPad, AttnDocMask> doc = {}) {
   using S = FaSmem<kD>;
   CUtensorMap tq, tk, tv;
   bool sq = false, sk = false, sv = false;
@@ -263,7 +284,7 @@ cudaError_t launch_fa(const AttnView& q, const AttnView& k, const AttnView& v, c
   ok &= make_tmap_bshd(&tk, k.ptr, dt, inner(k), Sk, B, (uint64_t)k.ss * 2, (uint64_t)k.sb * 2, 64, kFaKv, &sk);
   ok &= make_tmap_bshd(&tv, v.ptr, dt, inner(v), Sk, B, (uint64_t)v.ss * 2, (uint64_t)v.sb * 2, 64, 64, &sv);
   if (!ok) return cudaErrorInvalidValue;
-  auto kern = attention_fwd_kernel<kD, kCausal, kBf16, kGqa, kDoc>;
+  auto kern = attention_fwd_kernel<kD, kCausal, kBf16, kGqa, kDoc, kKeyPad>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal);
@@ -303,6 +324,13 @@ cudaError_t launch_fa_doc(const AttnView& q, const AttnView& k, const AttnView& 
                 : launch_fa<64, false, kBf16, kGqa, true>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, scale, drop, st, doc);
 }
 
+template <bool kBf16>
+cudaError_t launch_fa_keypad(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H,
+                             int D, float scale, AttnDropout drop, const AttnKeyPad& pad, cudaStream_t st) {
+  if (D == 128) return launch_fa<128, false, kBf16, false, false, true>(q, k, v, out, lse, B, Sq, Sk, H, H, scale, drop, st, pad);
+  return launch_fa<64, false, kBf16, false, false, true>(q, k, v, out, lse, B, Sq, Sk, H, H, scale, drop, st, pad);
+}
+
 }  // namespace
 
 cudaError_t attention_fwd_v2(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H,
@@ -330,6 +358,16 @@ cudaError_t attention_fwd_doc(const AttnView& q, const AttnView& k, const AttnVi
                       : launch_fa_doc<false, true>(q, k, v, out, lse, B, Sq, Sk, H, Hkv, D, scale, causal, drop, doc, st);
   return dtype == 1 ? launch_fa_doc<true, false>(q, k, v, out, lse, B, Sq, Sk, H, H, D, scale, causal, drop, doc, st)
                     : launch_fa_doc<false, false>(q, k, v, out, lse, B, Sq, Sk, H, H, D, scale, causal, drop, doc, st);
+}
+
+cudaError_t attention_fwd_keypad(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H,
+                                 int D, float scale, AttnDropout drop, const AttnKeyPad& pad, int dtype, cudaStream_t st) {
+  if ((D != 64 && D != 128) || (dtype != 0 && dtype != 1) || B < 1 || Sq < 1 || Sk < 1 || H < 1) return cudaErrorInvalidValue;
+  if (pad.key_bits == nullptr || pad.key_end == nullptr || pad.key_dense == nullptr) return cudaErrorInvalidValue;
+  for (const AttnView* t : {&q, &k, &v, &out})
+    if (t->ptr == nullptr || (reinterpret_cast<uintptr_t>(t->ptr) % 16) || t->sb % 8 || t->ss % 8 || t->sh % 8) return cudaErrorInvalidValue;
+  return dtype == 1 ? launch_fa_keypad<true>(q, k, v, out, lse, B, Sq, Sk, H, D, scale, drop, pad, st)
+                    : launch_fa_keypad<false>(q, k, v, out, lse, B, Sq, Sk, H, D, scale, drop, pad, st);
 }
 
 // ---- document-mask bounds: key_start[b, i] = clamp(i - pos[b, i], 0, i) (or clamp(src, 0, i) when src already holds key starts), and
@@ -413,6 +451,65 @@ cudaError_t attention_ring_doc_bounds(const int64_t* pos, int B, int s_l, int c,
   if (pos == nullptr || out == nullptr || B < 1 || B > 65535 || s_l < 2 || s_l % 2 || c < 1 || c > 65535 || r < 0 || r >= c)
     return cudaErrorInvalidValue;
   attn_ring_doc_bounds_kernel<<<dim3((s_l + 63) / 64, B, c), 64, 0, st>>>(pos, s_l, c, r, out);
+  return cudaGetLastError();
+}
+
+// ---- key-padding bounds: one 256-thread block per batch row, warp w takes the 32-key words w, w + 8, ... (one ballot per word).  kSrc as
+// the src_dtype of attention_key_pad_bounds; 16-bit floats are read as their bits (+-0 is the only zero).
+template <int kSrc, typename T>
+__global__ void attn_key_pad_bounds_kernel(const T* __restrict__ src, int from_ids, int64_t pad_id, int S, uint32_t* __restrict__ key_bits,
+                                           int* __restrict__ key_end, int* __restrict__ key_dense) {
+  __shared__ int red[2][8];
+  const int b = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int n_words = (S + 31) / 32;
+  uint32_t* row = key_bits + (size_t)b * n_words;
+  int last = -1, first_bad = S;                   // the last valid key, the first invalid one
+  for (int w = warp; w < n_words; w += 8) {
+    const int j = w * 32 + lane;
+    bool valid = false;
+    if (j < S) {
+      const T x = src[(size_t)b * S + j];
+      if constexpr (kSrc == 1 || kSrc == 2) valid = from_ids ? (int64_t)x != pad_id : x != 0;
+      else if constexpr (kSrc == 4 || kSrc == 5) valid = (x & 0x7FFFu) != 0;
+      else valid = x != 0;
+      last = valid ? j : last;
+      first_bad = valid ? first_bad : min(first_bad, j);
+    }
+    const uint32_t word = __ballot_sync(0xffffffffu, valid);
+    if (lane == 0) row[w] = word;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    last = max(last, __shfl_xor_sync(0xffffffffu, last, o));
+    first_bad = min(first_bad, __shfl_xor_sync(0xffffffffu, first_bad, o));
+  }
+  if (lane == 0) { red[0][warp] = last; red[1][warp] = first_bad; }
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < 8; ++i) { last = max(last, red[0][i]); first_bad = min(first_bad, red[1][i]); }
+  const bool empty = last < 0;                    // no valid key: every key of [0, S), which leaves the softmax of the additive mask unchanged
+  if (empty && lane == 0)
+    for (int w = warp; w < n_words; w += 8) row[w] = S - w * 32 >= 32 ? ~0u : (1u << (S - w * 32)) - 1u;
+  if (threadIdx.x == 0) {
+    key_end[b] = empty ? S : last + 1;
+    key_dense[b] = empty ? S : first_bad;
+  }
+}
+
+cudaError_t attention_key_pad_bounds(const void* src, int src_dtype, bool from_ids, int64_t pad_id, int B, int S, uint32_t* key_bits, int* key_end,
+                                     int* key_dense, cudaStream_t st) {
+  if (src == nullptr || key_bits == nullptr || key_end == nullptr || key_dense == nullptr || B < 1 || S < 1) return cudaErrorInvalidValue;
+  if (from_ids && src_dtype != 1 && src_dtype != 2) return cudaErrorInvalidValue;
+  const int f = from_ids ? 1 : 0;
+  switch (src_dtype) {
+    case 0: attn_key_pad_bounds_kernel<0><<<B, 256, 0, st>>>((const uint8_t*)src, f, pad_id, S, key_bits, key_end, key_dense); break;
+    case 1: attn_key_pad_bounds_kernel<1><<<B, 256, 0, st>>>((const int32_t*)src, f, pad_id, S, key_bits, key_end, key_dense); break;
+    case 2: attn_key_pad_bounds_kernel<2><<<B, 256, 0, st>>>((const int64_t*)src, f, pad_id, S, key_bits, key_end, key_dense); break;
+    case 3: attn_key_pad_bounds_kernel<3><<<B, 256, 0, st>>>((const float*)src, f, pad_id, S, key_bits, key_end, key_dense); break;
+    case 4: attn_key_pad_bounds_kernel<4><<<B, 256, 0, st>>>((const uint16_t*)src, f, pad_id, S, key_bits, key_end, key_dense); break;
+    case 5: attn_key_pad_bounds_kernel<5><<<B, 256, 0, st>>>((const uint16_t*)src, f, pad_id, S, key_bits, key_end, key_dense); break;
+    default: return cudaErrorInvalidValue;
+  }
   return cudaGetLastError();
 }
 

@@ -983,6 +983,87 @@ void attention_bwd_doc(const at::Tensor& q, const at::Tensor& k, const at::Tenso
                                         (float)scale, causal, pfx::AttnDropout{(float)dropout_p, (uint64_t)seed}, doc, dtype_code(q), cur_stream()));
 }
 
+// Key-padding mask from a [B, S] validity tensor (bool / uint8 / int32 / int64 / float32 / float16 / bfloat16, nonzero = valid) or, with
+// from_ids, from int32 / int64 ids (valid = id != pad_id): returns (key_bits int32 [B, ceil(S / 32)] holding the uint32 bit words,
+// key_end int32 [B], key_dense int32 [B]), computed by one kernel (see pfx::AttnKeyPad).
+std::vector<at::Tensor> attention_key_pad_bounds(const at::Tensor& src, bool from_ids, int64_t pad_id) {
+  TORCH_CHECK(src.is_cuda() && src.dim() == 2 && src.is_contiguous() && src.size(0) >= 1 && src.size(1) >= 1,
+              "attention_key_pad_bounds: contiguous [B, S] CUDA tensor with B, S >= 1");
+  int code = -1;
+  switch (src.scalar_type()) {
+    case at::kBool: case at::kByte: code = 0; break;
+    case at::kInt: code = 1; break;
+    case at::kLong: code = 2; break;
+    case at::kFloat: code = 3; break;
+    case at::kHalf: code = 4; break;
+    case at::kBFloat16: code = 5; break;
+    default: break;
+  }
+  TORCH_CHECK(code >= 0, "attention_key_pad_bounds: unsupported dtype ", src.scalar_type());
+  TORCH_CHECK(!from_ids || code == 1 || code == 2, "attention_key_pad_bounds: ids must be int32 or int64");
+  const c10::cuda::CUDAGuard guard(src.device());
+  const int64_t B = src.size(0), S = src.size(1);
+  auto i32 = src.options().dtype(at::kInt);
+  auto bits = at::empty({B, (S + 31) / 32}, i32), end = at::empty({B}, i32), dense = at::empty({B}, i32);
+  PFX_CUDA_CHECK(pfx::attention_key_pad_bounds(src.data_ptr(), code, from_ids, pad_id, (int)B, (int)S, reinterpret_cast<uint32_t*>(bits.data_ptr<int>()),
+                                               end.data_ptr<int>(), dense.data_ptr<int>(), cur_stream()));
+  return {bits, end, dense};
+}
+
+static pfx::AttnKeyPad attn_key_pad(const at::Tensor& bits, const at::Tensor& end, const at::Tensor& dense, int64_t B, int64_t Sk, const char* fn) {
+  for (const at::Tensor* t : {&bits, &end, &dense})
+    TORCH_CHECK(t->is_cuda() && t->is_contiguous() && t->scalar_type() == at::kInt, fn, ": key-padding bounds must be contiguous int32 CUDA tensors");
+  TORCH_CHECK(bits.numel() == B * ((Sk + 31) / 32) && end.numel() == B && dense.numel() == B, fn,
+              ": key-padding bounds must be [B, ceil(Sk / 32)], [B] and [B]");
+  return pfx::AttnKeyPad{reinterpret_cast<const uint32_t*>(bits.data_ptr<int>()), end.data_ptr<int>(), dense.data_ptr<int>()};
+}
+
+static void attn_check_mha(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v, const char* fn) {
+  TORCH_CHECK(q.dim() == 4 && k.dim() == 4 && k.sizes() == v.sizes() && q.size(0) == k.size(0) && q.size(2) == k.size(2) && q.size(3) == k.size(3),
+              fn, ": q [B,Sq,H,D] and k / v [B,Sk,H,D] with one head count");
+  TORCH_CHECK(q.size(3) == 64 || q.size(3) == 128, fn, ": head_dim must be 64 or 128");
+  TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type(), fn, ": q, k, v must have one dtype");
+}
+
+// Non-causal multi-head flash attention under a key-padding mask from attention_key_pad_bounds (bits over the Sk keys).  Views as in
+// attention_fwd_v2.
+std::vector<at::Tensor> attention_fwd_keypad(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v, const at::Tensor& key_bits,
+                                             const at::Tensor& key_end, const at::Tensor& key_dense, double scale, double dropout_p, int64_t seed) {
+  attn_check_mha(q, k, v, "attention_fwd_keypad");
+  const int64_t B = q.size(0), Sq = q.size(1), Sk = k.size(1), H = q.size(2), D = q.size(3);
+  const pfx::AttnKeyPad pad = attn_key_pad(key_bits, key_end, key_dense, B, Sk, "attention_fwd_keypad");
+  const c10::cuda::CUDAGuard guard(q.device());
+  auto out = at::empty({B, Sq, H, D}, q.options());
+  auto lse = at::empty({B, H, Sq}, q.options().dtype(at::kFloat));
+  PFX_CUDA_CHECK(pfx::attention_fwd_keypad(attn_view(q, "q"), attn_view(k, "k"), attn_view(v, "v"), attn_view(out, "out"), lse.data_ptr<float>(), (int)B,
+                                           (int)Sq, (int)Sk, (int)H, (int)D, (float)scale, pfx::AttnDropout{(float)dropout_p, (uint64_t)seed}, pad,
+                                           dtype_code(q), cur_stream()));
+  return {out, lse};
+}
+
+// Backward of attention_fwd_keypad: writes dq / dk / dv into the given (possibly strided) views; dk = dv = 0 on padded keys.
+void attention_bwd_keypad(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v, const at::Tensor& out, const at::Tensor& dout,
+                          const at::Tensor& lse, at::Tensor& dq, at::Tensor& dk, at::Tensor& dv, const at::Tensor& key_bits, const at::Tensor& key_end,
+                          const at::Tensor& key_dense, double scale, double dropout_p, int64_t seed) {
+  attn_check_mha(q, k, v, "attention_bwd_keypad");
+  const int64_t B = q.size(0), Sq = q.size(1), Sk = k.size(1), H = q.size(2), D = q.size(3);
+  TORCH_CHECK(k.sizes() == dk.sizes() && k.sizes() == dv.sizes() && q.sizes() == dq.sizes(), "attention_bwd_keypad: gradients must have the shapes of q / k / v");
+  TORCH_CHECK(out.sizes() == q.sizes() && dout.sizes() == q.sizes(), "attention_bwd_keypad: out / dout must be [B,Sq,H,D]");
+  TORCH_CHECK(lse.is_cuda() && lse.is_contiguous() && lse.scalar_type() == at::kFloat && lse.numel() == B * Sq * H, "attention_bwd_keypad: lse");
+  for (const at::Tensor* t : std::initializer_list<const at::Tensor*>{&out, &dout, &dq, &dk, &dv})
+    TORCH_CHECK(t->scalar_type() == q.scalar_type(), "attention_bwd_keypad: q, k, v, out, dout and the gradients must have one dtype");
+  const pfx::AttnKeyPad pad = attn_key_pad(key_bits, key_end, key_dense, B, Sk, "attention_bwd_keypad");
+  const c10::cuda::CUDAGuard guard(q.device());
+  const int64_t s_pad = (Sq + 63) / 64 * 64;
+  auto f32 = q.options().dtype(at::kFloat);
+  auto dq_acc = at::empty({B, Sq, H, D}, f32);
+  auto stats = at::empty({2, B * H * s_pad}, f32);
+  PFX_CUDA_CHECK(pfx::attention_bwd_keypad(attn_view(q, "q"), attn_view(k, "k"), attn_view(v, "v"), attn_view(out, "out"), attn_view(dout, "dout"),
+                                           lse.data_ptr<float>(), attn_view(dq, "dq"), attn_view(dk, "dk"), attn_view(dv, "dv"), dq_acc.data_ptr<float>(),
+                                           stats[0].data_ptr<float>(), stats[1].data_ptr<float>(), (int)B, (int)Sq, (int)Sk, (int)H, (int)D, (float)scale,
+                                           pfx::AttnDropout{(float)dropout_p, (uint64_t)seed}, pad, dtype_code(q), cur_stream()));
+}
+
 at::Tensor attention_decode_packed(const at::Tensor& qkv, at::Tensor& k, at::Tensor& v, c10::optional<at::Tensor> mask, const at::Tensor& write_idx,
                                    double scale) {
   // qkv [B,1,Hkv,G+2,D] (fused projection output: per K/V head its G queries, key and value; G = 1 is [B,1,H,3,D]); appends this step's
@@ -1244,6 +1325,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("attention_bwd_doc", &attention_bwd_doc, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("out"), py::arg("dout"), py::arg("lse"),
         py::arg("dq"), py::arg("dk"), py::arg("dv"), py::arg("key_start"), py::arg("tile_min"), py::arg("tile_max"), py::arg("scale"),
         py::arg("dropout_p"), py::arg("seed"), py::arg("causal") = true);
+  m.def("attention_key_pad_bounds", &attention_key_pad_bounds, py::arg("src"), py::arg("from_ids") = false, py::arg("pad_id") = 0);
+  m.def("attention_fwd_keypad", &attention_fwd_keypad);
+  m.def("attention_bwd_keypad", &attention_bwd_keypad);
   m.def("attention_decode", &attention_decode);
   m.def("attention_decode_packed", &attention_decode_packed);
   m.def("gemm_bias_gelu_dual", &gemm_bias_gelu_dual);

@@ -67,6 +67,28 @@ cudaError_t attention_bwd_doc(const AttnView& q, const AttnView& k, const AttnVi
                               int Sk, int H, int Hkv, int D, float scale, bool causal, AttnDropout drop, const AttnDocMask& doc, int dtype,
                               cudaStream_t st);
 
+// Key-padding mask for bidirectional attention: query i of batch row b attends key j iff bit j % 32 of key_bits[b, j / 32] is set (any
+// pattern).  key_end[b] = 1 + the last valid key: key tiles at or past it are never loaded.  key_dense[b] = the first invalid key (Sk
+// when there is none): key tiles entirely below it need no per-element compare.  A row with no valid key has every bit of [0, Sk) set
+// (softmax is unchanged by one additive constant on every logit), so key_end >= 1 always.  Bits at or past Sk are 0.
+struct AttnKeyPad {
+  const uint32_t* key_bits;  // [B, ceil(Sk / 32)]
+  const int* key_end;        // int32 [B]
+  const int* key_dense;      // int32 [B]
+};
+
+// Writes AttnKeyPad from a [B, S] tensor in one launch: valid = (src != pad_id) when from_ids, else (src != 0).
+// src_dtype: 0 = bool / uint8, 1 = int32, 2 = int64, 3 = float32, 4 = float16, 5 = bfloat16.
+cudaError_t attention_key_pad_bounds(const void* src, int src_dtype, bool from_ids, int64_t pad_id, int B, int S, uint32_t* key_bits, int* key_end,
+                                     int* key_dense, cudaStream_t st);
+
+// attention_fwd_v2 / attention_bwd, non-causal multi-head (H == Hkv), under a key-padding mask (separate kernel instantiations).
+cudaError_t attention_fwd_keypad(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, float* lse, int B, int Sq, int Sk, int H,
+                                 int D, float scale, AttnDropout drop, const AttnKeyPad& pad, int dtype, cudaStream_t st);
+cudaError_t attention_bwd_keypad(const AttnView& q, const AttnView& k, const AttnView& v, const AttnView& out, const AttnView& dout, const float* lse,
+                                 const AttnView& dq, const AttnView& dk, const AttnView& dv, float* dq_acc, float* lse2, float* delta, int B, int Sq,
+                                 int Sk, int H, int D, float scale, AttnDropout drop, const AttnKeyPad& pad, int dtype, cudaStream_t st);
+
 // Evoformer gated attention (head width 32, H even): softmax(scale QK^T + mask_bias[g, k] + pair_bias[g / groups_per_pair, h, q, k]) V * sigmoid(gate).
 // q / out / gate [G, Sq, H, 32], k / v [G, Sk, H, 32] bf16 contiguous; mask_bias fp32 [G, Sk]; pair_bias bf16; stats fp32 [2, G, H, Sq]: the
 // row maximum of the logits and log2 of the row sum relative to it (log2 units; log-sum-exp = (stats[0] + stats[1]) ln 2).

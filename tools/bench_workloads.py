@@ -41,6 +41,7 @@ def parse():
     p.add_argument("--mp", type=int, default=0, help="ernie: tensor-parallel degree (default 4 on 8 GPUs, else min(world, 2))")
     p.add_argument("--fp8", type=int, default=0, help="ernie: fp8 forward GEMMs in the tensor-parallel linears")
     p.add_argument("--sp", type=int, default=0, help="ernie: Megatron sequence parallelism over the tensor-parallel group")
+    p.add_argument("--pad", type=float, default=0.0, help="ernie: right-pad every row by this fraction of the sequence (pad id 0, mask 0)")
     p.add_argument("--fused-tp", type=int, default=0, help="ernie (with --sp 1): all-gather->GEMM / GEMM->reduce-scatter as single peer-memory kernels")
     return p.parse_args()
 
@@ -138,7 +139,8 @@ def main():
         cfg = C.get_config(os.path.join(CFG, "nlp/ernie/pretrain_ernie_10B_mp4_stage3_fp8.yaml"), ov, nranks=world)
         unit, per_step = "tokens/s", local * seq * sh
         name = (f"ERNIE 10B-class (h4096 L{cfg.Model.num_hidden_layers}), mp{mp} x ZeRO-3 sharding{sh}, {'fp8' if a.fp8 else 'bf16'} TP GEMMs"
-                + (", sequence parallel" if a.sp else "") + (" with fused GEMM+collective kernels" if (a.fused_tp and a.sp) else ""))
+                + (", sequence parallel" if a.sp else "") + (" with fused GEMM+collective kernels" if (a.fused_tp and a.sp) else "")
+                + (f", rows right-padded by {a.pad:.0%}" if a.pad else ""))
         vocab = cfg.Model.vocab_size
         n_mask = 76
 
@@ -146,7 +148,10 @@ def main():
             ids = torch.randint(4, vocab, (local, seq), generator=g)
             seg = torch.zeros(local, seq, dtype=torch.long)
             mask = torch.ones(local, seq, dtype=torch.float32)
-            pos = torch.stack([torch.randperm(seq, generator=g)[:n_mask].sort().values + i * seq for i in range(local)]).reshape(-1)
+            n_valid = seq - int(a.pad * seq)
+            mask[:, n_valid:] = 0.0
+            ids[:, n_valid:] = 0
+            pos = torch.stack([torch.randperm(n_valid, generator=g)[:n_mask].sort().values + i * seq for i in range(local)]).reshape(-1)
             labels = torch.randint(4, vocab, (local * n_mask,), generator=g)
             return [ids, seg, mask, pos, labels, torch.randint(0, 2, (local,), generator=g)]
 
