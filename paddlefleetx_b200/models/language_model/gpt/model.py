@@ -8,7 +8,7 @@ Capabilities mirrored from the reference (single-card ``gpt/dygraph/single_model
   * recompute granularities ``full | full_attn | core_attn`` and ``no_recompute_layers``,
   * Megatron TP (+ sequence parallel in ``[s, b, h]`` layout) through ``parallel/tp_layers.py``,
   * KV cache for generation, sequence-classification head, masked-mean pre-training criterion,
-  * optional MoE FFN per layer (``moe_configs``).
+  * optional MoE FFN per layer (``moe_configs``), with GELU or SwiGLU experts (``ffn_activation``).
 
 State-dict keys keep the reference's structured names (SURVEY §5.4), e.g.
 ``gpt.decoder.layers.3.self_attn.qkv_proj.weight``; linear weights are stored ``[out, in]`` (torch) instead
@@ -330,8 +330,6 @@ class TransformerDecoderLayer(nn.Module):
         super().__init__()
         if ffn_activation not in FFN_ACTIVATIONS:
             raise ValueError(f"Model.ffn_activation must be one of {', '.join(FFN_ACTIVATIONS)}, got {ffn_activation!r}")
-        if ffn_activation == "swiglu" and moe_layer is not None:
-            raise ValueError("ffn_activation: swiglu is not supported with MoE layers (moe_configs); the experts keep GELU")
         self.ffn_activation = ffn_activation
         out_std = init_std / math.sqrt(2.0 * num_layers)
         self.sequence_parallel = sequence_parallel
@@ -493,7 +491,8 @@ class GPTModel(nn.Module):
             if moe_configs and moe_configs.get("expert_mode", False):
                 from ..moe.moe_layer import build_moe_layer
 
-                moe = build_moe_layer(hidden_size, ffn_hidden_size, moe_configs, num_layers, initializer_range, mp_group, dtype, device, i)
+                moe = build_moe_layer(hidden_size, ffn_hidden_size, moe_configs, num_layers, initializer_range, mp_group, dtype, device, i,
+                                      ffn_activation)
             layers.append(TransformerDecoderLayer(
                 hidden_size, num_attention_heads, ffn_hidden_size, hidden_dropout_prob, attention_probs_dropout_prob, num_layers,
                 sequence_parallel=sp, mp_group=mp_group, init_std=initializer_range,

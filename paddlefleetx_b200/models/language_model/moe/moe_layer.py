@@ -26,12 +26,18 @@ from .utils import count_by_gate
 
 
 class ExpertLayer(nn.Module):
-    """h -> 4h -> GELU(tanh) -> h; parameters tagged ``is_expert`` (excluded from dp/mp broadcast, clipped with the
+    """h -> 4h -> GELU(tanh) -> h, or with ``activation="swiglu"`` the gated FFN of width ``d_hidden`` = F: ``htoh4`` is [2F, h] with
+    pair-interleaved rows (2i the gate channel i, 2i + 1 its up channel, as the dense GPT's ``linear1``) and ``h4toh`` is [h, F], so the
+    checkpoint keys stay those of a GELU expert.  Parameters are tagged ``is_expert`` (excluded from dp/mp broadcast, clipped with the
     expert-group norm) — the reference tags by renaming params with an ``expert_`` prefix (single_model.py:71-74)."""
 
-    def __init__(self, d_model: int, d_hidden: int, init_std: float = 0.02, out_std: Optional[float] = None, dtype=None, device=None):
+    def __init__(self, d_model: int, d_hidden: int, init_std: float = 0.02, out_std: Optional[float] = None, dtype=None, device=None,
+                 activation: str = "gelu"):
         super().__init__()
-        self.htoh4 = nn.Linear(d_model, d_hidden, dtype=dtype, device=device)
+        if activation not in ("gelu", "swiglu"):
+            raise ValueError(f"ExpertLayer activation must be gelu or swiglu, got {activation!r}")
+        self.activation = activation
+        self.htoh4 = nn.Linear(d_model, 2 * d_hidden if activation == "swiglu" else d_hidden, dtype=dtype, device=device)
         self.h4toh = nn.Linear(d_hidden, d_model, dtype=dtype, device=device)
         with torch.no_grad():
             self.htoh4.weight.normal_(0.0, init_std); self.htoh4.bias.zero_()
@@ -41,6 +47,8 @@ class ExpertLayer(nn.Module):
             p.no_sync = True
 
     def forward(self, x):
+        if self.activation == "swiglu":
+            return OF.linear(OF.bias_swiglu(OF.linear(x, self.htoh4.weight), self.htoh4.bias), self.h4toh.weight, self.h4toh.bias)
         return OF.fused_ffn(x, self.htoh4.weight, self.htoh4.bias, self.h4toh.weight, self.h4toh.bias)
 
 
@@ -182,14 +190,14 @@ class MoELayer(nn.Module):
 
 
 def build_moe_layer(hidden: int, ffn_hidden: int, moe_configs: dict, num_layers: int, init_std: float, mp_group, dtype, device,
-                    layer_idx: int = 0) -> MoELayer:
+                    layer_idx: int = 0, ffn_activation: str = "gelu") -> MoELayer:
     from ....distributed.apis import env
 
     hcg = env.get_hcg()
     moe_group = hcg.get_moe_group() if env.world_size() > 1 else None
     n = int(moe_configs.get("num_experts", 1))
     out_std = init_std / math.sqrt(2.0 * num_layers)
-    experts = [ExpertLayer(hidden, ffn_hidden, init_std, out_std, dtype, device) for _ in range(n)]
+    experts = [ExpertLayer(hidden, ffn_hidden, init_std, out_std, dtype, device, ffn_activation) for _ in range(n)]
     gate_cfg = {"type": moe_configs.get("gate", "gshard"), "top_k": int(moe_configs.get("top_k", 2))}
     return MoELayer(hidden, experts, gate=gate_cfg, moe_group=moe_group, mp_group=mp_group if C.group_size(mp_group) > 1 else None,
                     recompute_interval=int(moe_configs.get("recompute_interval", 0)), dtype=dtype, device=device,

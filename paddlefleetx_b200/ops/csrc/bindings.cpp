@@ -1188,6 +1188,8 @@ std::vector<at::Tensor> moe_tile_table(const at::Tensor& seg, int64_t e_local, i
 
 // Grouped expert GEMM, rows grouped: d[r, :] = a[r, :] . B[g(r)]^T (+ bias[g(r)]) for the expert g(r) that owns row block r / 128.
 //   b: [G, N, K] (b_kmajor: forward) or [G, K, N] (dgrad).  epilogue: EPI_NONE / EPI_BIAS / EPI_BIAS_GELU_DUAL (out2) / EPI_DGELU (aux).
+//   SwiGLU experts (pair-interleaved gate / up columns, width F): EPI_BIAS_SWIGLU_DUAL (forward, N = 2F: out = pre [M, 2F], out2 = h [M, F])
+//   and EPI_DSWIGLU (dgrad, N = F: aux = pre [M, 2F], out = dpre [M, 2F]).
 at::Tensor gemm_grouped(const at::Tensor& a, const at::Tensor& b, c10::optional<at::Tensor> bias, const at::Tensor& tile_group, at::Tensor& out,
                         bool b_kmajor, int64_t epilogue, c10::optional<at::Tensor> out2, c10::optional<at::Tensor> aux, int64_t row_align) {
   TORCH_CHECK(a.is_cuda() && a.dim() == 2 && b.dim() == 3 && a.is_contiguous() && b.is_contiguous() && out.is_contiguous(), "gemm_grouped: a [M,K], b [G,*,*] contiguous");
@@ -1196,26 +1198,37 @@ at::Tensor gemm_grouped(const at::Tensor& a, const at::Tensor& b, c10::optional<
   const int64_t N = b_kmajor ? b.size(1) : b.size(2);
   TORCH_CHECK((b_kmajor ? b.size(2) : b.size(1)) == K, "gemm_grouped: K mismatch");
   TORCH_CHECK(M % 128 == 0 && tile_group.numel() == M / 128 && tile_group.scalar_type() == at::kInt, "gemm_grouped: tile table must cover M / 128 blocks");
-  TORCH_CHECK(out.dim() == 2 && out.size(0) == M && out.size(1) == N && N % 8 == 0 && K % 64 == 0, "gemm_grouped: out [M, N], N % 8 == 0, K % 64 == 0");
+  const bool dswiglu = epilogue == pfx::EPI_DSWIGLU;
+  const int64_t out_cols = dswiglu ? 2 * N : N;      // dSwiGLU: a (dg, du) pair per column of dh
+  TORCH_CHECK(out.dim() == 2 && out.size(0) == M && out.size(1) == out_cols && N % 8 == 0 && K % 64 == 0,
+              "gemm_grouped: out [M, ", out_cols, "], N % 8 == 0, K % 64 == 0; got out ", out.sizes(), ", N ", N, ", K ", K);
+  if (epilogue == pfx::EPI_BIAS_SWIGLU_DUAL) TORCH_CHECK(b_kmajor && N % 16 == 0, "gemm_grouped: SwiGLU forward needs a K-major b [G, 2F, K], 2F % 16 == 0");
+  if (dswiglu) TORCH_CHECK(!b_kmajor, "gemm_grouped: dSwiGLU needs an MN-major b [G, K, F]");
   const c10::cuda::CUDAGuard guard(a.device());
   pfx::GemmArgs g{};
   g.a = a.data_ptr(); g.b = b.data_ptr(); g.d = out.data_ptr();
   if (bias.has_value() && bias->defined()) {
     TORCH_CHECK(bias->scalar_type() == a.scalar_type() && bias->numel() == G * N && bias->is_contiguous(), "gemm_grouped: bias [G, N] of the operands' dtype");
+    TORCH_CHECK(!dswiglu, "gemm_grouped: dSwiGLU takes no bias");
     g.bias = bias->data_ptr();
   } else {
-    TORCH_CHECK(epilogue == pfx::EPI_NONE || epilogue == pfx::EPI_DGELU, "gemm_grouped: bias epilogue without bias");
+    TORCH_CHECK(epilogue == pfx::EPI_NONE || epilogue == pfx::EPI_DGELU || dswiglu, "gemm_grouped: bias epilogue without bias");
   }
   if (epilogue == pfx::EPI_BIAS_GELU_DUAL) {
     TORCH_CHECK(out2.has_value() && out2->is_contiguous() && out2->sizes() == out.sizes() && out2->scalar_type() == a.scalar_type(), "gemm_grouped: out2 like out");
     g.d2 = out2->data_ptr();
   }
-  if (epilogue == pfx::EPI_DGELU) {
+  if (epilogue == pfx::EPI_BIAS_SWIGLU_DUAL) {
+    TORCH_CHECK(out2.has_value() && out2->is_contiguous() && out2->dim() == 2 && out2->size(0) == M && out2->size(1) == N / 2 &&
+                out2->scalar_type() == a.scalar_type(), "gemm_grouped: SwiGLU out2 [M, ", N / 2, "] of the operands' dtype");
+    g.d2 = out2->data_ptr();
+  }
+  if (epilogue == pfx::EPI_DGELU || dswiglu) {
     TORCH_CHECK(aux.has_value() && aux->is_contiguous() && aux->sizes() == out.sizes() && aux->scalar_type() == a.scalar_type(), "gemm_grouped: aux like out");
-    g.aux = aux->data_ptr(); g.ld_aux = (int)N;
+    g.aux = aux->data_ptr(); g.ld_aux = (int)out_cols;
   }
   g.M = (int)M; g.N = (int)N; g.K = (int)K;
-  g.lda = (int)K; g.ldb = (int)(b_kmajor ? K : N); g.ldd = (int)N;
+  g.lda = (int)K; g.ldb = (int)(b_kmajor ? K : N); g.ldd = (int)out_cols;
   g.a_kmajor = true; g.b_kmajor = b_kmajor; g.out_mode = 0; g.epilogue = (int)epilogue; g.ab_format = dtype_code(a); g.num_sms = num_sms(); g.config = 0;
   g.group.mode = 1; g.group.tile_group = tile_group.data_ptr<int>(); g.group.groups = (int)G; g.group.b_group_stride = (int)(b_kmajor ? N : K);
   g.group.row_align = (int)row_align;

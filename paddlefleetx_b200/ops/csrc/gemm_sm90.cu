@@ -136,7 +136,12 @@ __device__ void ag_push_role(const GemmComm& c, int comm_cta, int num_comm_ctas,
 // pre-activation of EPI_DGELU) loads are bf16, otherwise fp16.  The form must be a compile-time choice: a runtime branch between two
 // wgmma forms puts every wgmma of the k-block in its own branch arm, and ptxas then fences and waits on each one separately (C7519).
 // kOutMode: 0 = bf16/fp16 via TMA store, 1 = fp32 direct store, 2 = fp32 direct accumulate (D += acc),
-//           3 = bf16 scatter into the destination rank's staging buffer over NVLink (GEMM -> reduce-scatter)
+//           3 = bf16 scatter into the destination rank's staging buffer over NVLink (GEMM -> reduce-scatter),
+//           4 / 5 = the 16-bit TMA-store outputs of EPI_BIAS_SWIGLU_DUAL / EPI_DSWIGLU (kOutSwiGLU / kOutDSwiGLU; the launcher picks them from
+//           the epilogue, GemmArgs::out_mode stays 0).  They are modes of their own, not runtime epilogue branches, so the instantiations
+//           of modes 0-3 keep their registers: the 128 x 128 kernel sits at 162-168 of them.
+constexpr int kOutSwiGLU = 4, kOutDSwiGLU = 5;
+
 template <int kBlockN, bool kAK, bool kBK, int kOutMode, bool kBf16>
 __global__ void __launch_bounds__(GemmSmem<kBlockN>::kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
@@ -186,7 +191,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   if (warp == 8 && elect_one()) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
-    if (kOutMode == 0) tma_prefetch_desc(&tmap_d);
+    if (kOutMode == 0 || kOutMode >= kOutSwiGLU) tma_prefetch_desc(&tmap_d);
     if (kOutMode == 3) { for (int i = 0; i < comm.world; ++i) tma_prefetch_desc(&peer_maps.m[i]); }
     for (int s = 0; s < kStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kNumConsumerWarps); }
     fence_barrier_init();
@@ -291,6 +296,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         tile_k_blocks = __ldg(grp.seg + 2 * ((tc.m_blk * kBlockM) / grp.m_per_group) + 1) / kBlockK;
       }
       const bool empty_k = tile_k_blocks == 0;   // K-grouped tile of an expert without tokens: the accumulator was never written, the result is zero
+      if constexpr (kOutMode == kOutDSwiGLU) {
+        // the epilogue reads this tile's pre-activation [128 rows, 2 x 128 columns]: start pulling it into L2 now, under the mainloop
+        // (the 4 threads of a row take 128 bytes each)
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int grow = row0 + (int)row_lo + 8 * hh;
+          if (grow < M && col_tile + (int)(lane & 3u) * 32 < N)
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(aux + (size_t)grow * ld_aux + 2 * col_tile + (lane & 3u) * 64u));
+        }
+      }
       int prev_stage = -1;
       for (int kb = 0; kb < tile_k_blocks; ++kb) {
         mbar_wait(full_bar(stage), phase);
@@ -327,7 +342,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 #pragma unroll
           for (int i = 0; i < 32; ++i) v[i] = empty_k ? 0.f : acc[c * 32 + i];
         }
-        if (epilogue == EPI_BIAS || epilogue == EPI_BIAS_GELU || epilogue == EPI_BIAS_GELU_DUAL) {
+        if (kOutMode == kOutSwiGLU || (kOutMode != kOutDSwiGLU && (epilogue == EPI_BIAS || epilogue == EPI_BIAS_GELU || epilogue == EPI_BIAS_GELU_DUAL))) {
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             if (cb + 8 * j < N) {   // N % 8 == 0 is required by the host wrapper
@@ -336,11 +351,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             }
           }
         }
-        if (!S::kWide && (epilogue == EPI_BIAS_GELU || epilogue == EPI_GELU)) {   // the wide tile serves EPI_NONE / EPI_BIAS / EPI_DGELU
+        if (!S::kWide && kOutMode < kOutSwiGLU && (epilogue == EPI_BIAS_GELU || epilogue == EPI_GELU)) {   // the wide tile serves EPI_NONE / EPI_BIAS / EPI_DGELU
 #pragma unroll
           for (int i = 0; i < 32; ++i) v[i] = gelu_tanh(v[i]);
         }
-        if (epilogue == EPI_DGELU) {      // acc * gelu'(saved pre-activation)
+        if (kOutMode < kOutSwiGLU && epilogue == EPI_DGELU) {      // acc * gelu'(saved pre-activation)
 #pragma unroll
           for (int hh = 0; hh < 2; ++hh) {
             const int grow_aux = row0 + (int)row_lo + 8 * hh;
@@ -356,18 +371,39 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             }
           }
         }
-        if constexpr (kOutMode == 0 || kOutMode == 3) {
-          // pack v[] into the swizzled staging buffer and TMA-store it; called twice per chunk by the dual-output epilogue
-          auto store_chunk = [&](const CUtensorMap* map_d) {
+        if constexpr (kOutMode != 1 && kOutMode != 2) {
+          // fill(box) writes one store box into the next staging buffer, which is then TMA-stored at column x of the tile's rows; called
+          // twice per chunk by the dual-output and dSwiGLU epilogues
+          auto store_box = [&](const CUtensorMap* map_d, int x, auto&& fill) {
           const uint32_t buf = store_iter & 1u;
           if (store_iter >= 2) {
             if (is_store_thread) tma_store_wait_read<1>();
             asm volatile("bar.sync 1, 256;" ::: "memory");
           }
+          fill(smem_epi + buf * S::kEpiBytes);
+          fence_proxy_async_smem();
+          asm volatile("bar.sync 1, 256;" ::: "memory");
+          if (is_store_thread) {
+            if (col0 < N && row0 < M) {
+              if constexpr (kOutMode == 3) {
+                // tile -> owner rank's staging slot [my_rank] through its NVLink-mapped address (TMA store to peer memory)
+                const int dst_rank = row0 / comm.rows_per_rank;
+                tma_store_2d(&peer_maps.m[dst_rank], smem_epi + buf * S::kEpiBytes, x,
+                             comm.my_rank * comm.rows_per_rank + (row0 - dst_rank * comm.rows_per_rank));
+              } else {
+                tma_store_2d(map_d, smem_epi + buf * S::kEpiBytes, x, row0);
+              }
+            }
+            tma_store_commit();
+          }
+          ++store_iter;
+          };
+          // v[] packed into a 64-column box with the 128-byte swizzle
+          auto fill_v = [&](uint32_t box) {
 #pragma unroll
           for (int hh = 0; hh < 2; ++hh) {
             const uint32_t r = row_lo + 8u * hh;
-            uint32_t sbase = smem_epi + buf * S::kEpiBytes + r * 128u + col_in8 * 2u;
+            uint32_t sbase = box + r * 128u + col_in8 * 2u;
             uint32_t r_sw = r & 7u;
             // Wide tile: the compiler would keep the 16 swizzled store addresses live across the tile loop, and beside 128 accumulators
             // they spill.  Opaque copies make it form them anew for each chunk (a few integer ops).
@@ -378,28 +414,71 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
               asm volatile("st.shared.b32 [%0], %1;" ::"r"(sbase + (((uint32_t)j ^ r_sw) << 4)), "r"(p) : "memory");
             }
           }
-          fence_proxy_async_smem();
-          asm volatile("bar.sync 1, 256;" ::: "memory");
-          if (is_store_thread) {
-            if (col0 < N && row0 < M) {
-              if constexpr (kOutMode == 3) {
-                // tile -> owner rank's staging slot [my_rank] through its NVLink-mapped address (TMA store to peer memory)
-                const int dst_rank = row0 / comm.rows_per_rank;
-                tma_store_2d(&peer_maps.m[dst_rank], smem_epi + buf * S::kEpiBytes, col0,
-                             comm.my_rank * comm.rows_per_rank + (row0 - dst_rank * comm.rows_per_rank));
-              } else {
-                tma_store_2d(map_d, smem_epi + buf * S::kEpiBytes, col0, row0);
-              }
-            }
-            tma_store_commit();
-          }
-          ++store_iter;
           };
-          store_chunk(&tmap_d);
-          if (!S::kWide && epilogue == EPI_BIAS_GELU_DUAL) {
+          if constexpr (kOutMode == kOutDSwiGLU) {
+            // v = dh at columns f = cb + 8 j (+ 1) of [M, F]; the pair (dg, du) of f lands at columns 2 f, 2 f + 1 of [M, 2F], so this chunk's
+            // 64 columns of dh fill the 128 output columns from 2 col0 on: two boxes, j = 0-3 and j = 4-7.  Each thread reads and writes 4
+            // adjacent 16-bit values (8 bytes) per j and row.  The reads are all issued here, ahead of the staging-buffer barriers, which
+            // no load may cross: one wait for the chunk instead of one per box.
+            uint2 pv[2][8];   // (a, b) of f, (a, b) of f + 1, packed 16-bit
 #pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = gelu_tanh(v[i]);
-            store_chunk(&tmap_d2);
+            for (int hh = 0; hh < 2; ++hh) {
+              const int grow = row0 + (int)row_lo + 8 * hh;
+              const uint16_t* ap = aux + (size_t)grow * ld_aux + 2 * cb;
+#pragma unroll
+              for (int j = 0; j < 8; ++j)   // N % 8 == 0: f + 1 < N as well
+                pv[hh][j] = grow < M && cb + 8 * j < N ? __ldg(reinterpret_cast<const uint2*>(ap + 16 * j)) : make_uint2(0u, 0u);
+            }
+#pragma unroll
+            for (int half = 0; half < 2; ++half) {
+              store_box(&tmap_d, 2 * col0 + half * kStoreCols, [&](uint32_t box) {
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                  const uint32_t r = row_lo + 8u * hh;
+#pragma unroll
+                  for (int jj = 0; jj < 4; ++jj) {
+                    const int j = half * 4 + jj;
+                    const float2 p0 = unpack_16x2<kBf16>(pv[hh][j].x), p1 = unpack_16x2<kBf16>(pv[hh][j].y);
+                    const float pa[2] = {p0.x, p1.x}, pb[2] = {p0.y, p1.y};
+                    float o[4];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                      const float a = pa[e], b = pb[e], dh = v[4 * j + 2 * hh + e], s = swiglu_sigmoid(a);
+                      o[2 * e] = dh * b * s * (1.f + a * (1.f - s));
+                      o[2 * e + 1] = dh * a * s;
+                    }
+                    // 16-byte group 2 jj + (lane & 3) / 2 of the box row, its half (lane & 1)
+                    const uint32_t addr = box + r * 128u + (((2u * jj + ((lane & 3u) >> 1)) ^ (r & 7u)) << 4) + (lane & 1u) * 8u;
+                    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(pack_16x2<kBf16>(o[0], o[1])),
+                                 "r"(pack_16x2<kBf16>(o[2], o[3])) : "memory");
+                  }
+                }
+              });
+            }
+          } else {
+            store_box(&tmap_d, col0, fill_v);
+            if constexpr (kOutMode == kOutSwiGLU) {
+              // h = a s b of the fp32 pre-activation: v[4 j + 2 hh] / v[4 j + 2 hh + 1] are the gate / up of channel (cb + 8 j) / 2, so every
+              // thread holds whole pairs and a chunk of 64 pre-activation columns gives 32 columns of h.  They go out as a 32-column box of
+              // their own, unswizzled (64-byte rows), in half of a staging buffer.  Pairing two chunks into one 64-column box would keep 16
+              // more values live across the chunk loop, or need a third staging buffer; the single 16-bit stores here cost less.
+              store_box(&tmap_d2, col0 / 2, [&](uint32_t box) {
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                  const uint32_t rbase = box + (row_lo + 8u * hh) * 64u + col_in8;   // h column (lane & 3) + 4 j: byte 2 (lane & 3) + 8 j
+#pragma unroll
+                  for (int j = 0; j < 8; ++j) {
+                    const float a = v[4 * j + 2 * hh], b = v[4 * j + 2 * hh + 1];
+                    const uint16_t hv = (uint16_t)(pack_16x2<kBf16>(a * swiglu_sigmoid(a) * b, 0.f) & 0xffffu);
+                    asm volatile("st.shared.b16 [%0], %1;" ::"r"(rbase + 8u * j), "h"(hv) : "memory");
+                  }
+                }
+              });
+            } else if (!S::kWide && epilogue == EPI_BIAS_GELU_DUAL) {
+#pragma unroll
+              for (int i = 0; i < 32; ++i) v[i] = gelu_tanh(v[i]);
+              store_box(&tmap_d2, col0, fill_v);
+            }
           }
         } else {
 #pragma unroll
@@ -423,7 +502,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         }
       }
     }
-    if ((kOutMode == 0 || kOutMode == 3) && is_store_thread) tma_store_wait<0>();
+    if (kOutMode != 1 && kOutMode != 2 && is_store_thread) tma_store_wait<0>();
   }
 }
 
@@ -575,14 +654,20 @@ static cudaError_t launch_cfg(const GemmArgs& g, cudaStream_t stream) {
   else     ok &= make_tmap_2d(&ta, g.a, 2, dt, a_mn, g.K, (uint64_t)g.lda * 2, 64, kBlockK);
   if (kBK) ok &= make_tmap_2d(&tb, g.b, 2, dt, g.K, b_outer_k, (uint64_t)g.ldb * 2, kBlockK, kBlockN);
   else     ok &= make_tmap_2d(&tb, g.b, 2, dt, g.N, b_outer_mn, (uint64_t)g.ldb * 2, 64, kBlockK);
-  if (kOutMode == 0) ok &= make_tmap_2d(&td, g.d, 2, dt, g.N, g.M, (uint64_t)g.ldd * 2, kStoreCols, kBlockM);
+  const uint64_t d_cols = kOutMode == kOutDSwiGLU ? 2ull * g.N : (uint64_t)g.N;   // dSwiGLU writes a (dg, du) pair per column of dh
+  if (kOutMode == 0 || kOutMode >= kOutSwiGLU) ok &= make_tmap_2d(&td, g.d, 2, dt, d_cols, g.M, (uint64_t)g.ldd * 2, kStoreCols, kBlockM);
   else td = ta;
   CUtensorMap td2 = td;
   if (g.epilogue == EPI_BIAS_GELU_DUAL) {
     if (kOutMode != 0 || g.d2 == nullptr || g.bias == nullptr) return gemm_reject(g, kBlockN, __LINE__);
     ok &= make_tmap_2d(&td2, g.d2, 2, dt, g.N, g.M, (uint64_t)g.ldd * 2, kStoreCols, kBlockM);
   }
-  if (g.epilogue == EPI_DGELU && (g.aux == nullptr || g.ld_aux % 8 || (reinterpret_cast<uintptr_t>(g.aux) & 15))) return gemm_reject(g, kBlockN, __LINE__);
+  if (kOutMode == kOutSwiGLU) {   // h [M, N / 2], dense rows, stored 32 columns at a time without swizzle (see the kernel)
+    if (g.d2 == nullptr || g.bias == nullptr || g.N % 16) return gemm_reject(g, kBlockN, __LINE__);
+    ok &= make_tmap_2d_plain(&td2, g.d2, dt, g.N / 2, g.M, (uint64_t)g.N, kStoreCols / 2, kBlockM);
+  }
+  if ((g.epilogue == EPI_DGELU || kOutMode == kOutDSwiGLU) && (g.aux == nullptr || g.ld_aux % 8 || (reinterpret_cast<uintptr_t>(g.aux) & 15)))
+    return gemm_reject(g, kBlockN, __LINE__);
   PeerMaps pm;
   for (int i = 0; i < 8; ++i) pm.m[i] = ta;
   if (kOutMode == 3) {
@@ -649,6 +734,12 @@ static cudaError_t launch_out(const GemmArgs& g, cudaStream_t s) {
 
 cudaError_t gemm_wgmma(const GemmArgs& g, cudaStream_t stream) {
   if (g.M <= 0 || g.N <= 0 || g.K <= 0) return cudaSuccess;
+  // The SwiGLU epilogues exist for the grouped expert GEMMs only: FFN1 (A, B K-major) and the FFN2 dgrad (A K-major, B MN-major).
+  if (g.epilogue == EPI_BIAS_SWIGLU_DUAL || g.epilogue == EPI_DSWIGLU) {
+    const bool fwd = g.epilogue == EPI_BIAS_SWIGLU_DUAL;
+    if (g.config != 0 || g.out_mode != 0 || g.group.mode != 1 || !g.a_kmajor || g.b_kmajor != fwd) return gemm_reject(g, 128, __LINE__);
+    return fwd ? launch_cfg<128, true, true, kOutSwiGLU>(g, stream) : launch_cfg<128, true, false, kOutDSwiGLU>(g, stream);
+  }
   // The wide tile is compiled for the plain GEMM with a 16-bit output and the epilogues of the backward pass; any other request runs
   // 128 x 128 and gives the same result.
   const bool wide = g.config == 1 && g.out_mode == 0 && g.group.mode == 0 && g.comm.rows_per_rank == 0 && g.comm.ag_world <= 1 &&

@@ -331,9 +331,7 @@ cudaError_t bias_gelu(const void* x, const void* bias, const void* dy, void* out
 //   fwd  h  = a s b
 //   bwd  dg = dh b s (1 + a (1 - s)),   du = dh a s
 // A saturated gate stays finite: __expf(-a) overflows to inf for a < -88, s = 1 / inf = 0 and every product above is 0 (1 - s is formed
-// directly, never as e s, which would be inf * 0).
-__device__ __forceinline__ float swiglu_sigmoid(float a) { return 1.f / (1.f + __expf(-a)); }
-
+// directly, never as e s, which would be inf * 0).  s is swiglu_sigmoid (pfx_ptx.cuh), shared with the grouped GEMM's SwiGLU epilogues.
 template <typename T, bool kBwd>
 __global__ void bias_swiglu_kernel(const T* __restrict__ z, const T* __restrict__ bias, const T* __restrict__ dh, T* __restrict__ out,
                                    size_t total_vec, int nvec_row) {

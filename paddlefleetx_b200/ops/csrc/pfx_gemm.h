@@ -8,7 +8,14 @@ namespace pfx {
 
 // EPI_BIAS_GELU_DUAL: D = acc + bias (the pre-activation the backward needs) AND D2 = gelu(D), two TMA stores per tile (FFN1 forward).
 // EPI_DGELU:          D = acc * gelu'(aux) with aux = the saved pre-activation [M, N] (FFN2 dgrad producing dL/d(pre-activation)).
-enum Epilogue : int { EPI_NONE = 0, EPI_BIAS = 1, EPI_BIAS_GELU = 2, EPI_GELU = 3, EPI_BIAS_GELU_DUAL = 4, EPI_DGELU = 5 };
+// The SwiGLU pair (grouped mode 1 only, 128 x 128 tiles, 16-bit out mode 0); columns 2i / 2i + 1 of a [., 2F] tensor are the gate / up
+// channel i, a = gate, b = up, s = sigmoid(a):
+// EPI_BIAS_SWIGLU_DUAL: N = 2F, A and B K-major.  D = acc + bias [M, 2F] (the pre-activation) AND D2 = a s b [M, F] (FFN1 forward).
+// EPI_DSWIGLU:          N = F, A K-major, B MN-major; acc = dh.  aux = the saved pre-activation [M, 2F]; D [M, 2F] = (dh b s (1 + a (1 - s)),
+//                       dh a s) per pair (FFN2 dgrad producing dL/d(pre-activation)).
+enum Epilogue : int {
+  EPI_NONE = 0, EPI_BIAS = 1, EPI_BIAS_GELU = 2, EPI_GELU = 3, EPI_BIAS_GELU_DUAL = 4, EPI_DGELU = 5, EPI_BIAS_SWIGLU_DUAL = 6, EPI_DSWIGLU = 7
+};
 
 // Peer-memory communication descriptor of the fused GEMM+collective modes (passed to the kernel by value).
 struct GemmComm {
@@ -47,8 +54,8 @@ struct GemmArgs {
   const void* b;     // K-major: [N, K] row-major;                              MN-major: [K, N]
   void* d;           // [M, N] row-major, ldd = row stride (elements)
   const void* bias;  // [N] bf16 or nullptr
-  void* d2 = nullptr;         // EPI_BIAS_GELU_DUAL: second output [M, N] (same dtype / ldd as d)
-  const void* aux = nullptr;  // EPI_DGELU: pre-activation [M, N] (same dtype as the operands), row stride ld_aux
+  void* d2 = nullptr;         // EPI_BIAS_GELU_DUAL: second output [M, N] (same dtype / ldd as d); EPI_BIAS_SWIGLU_DUAL: [M, N / 2], dense
+  const void* aux = nullptr;  // EPI_DGELU: pre-activation [M, N] (same dtype as the operands), row stride ld_aux; EPI_DSWIGLU: [M, 2 N]
   int ld_aux = 0;
   int M, N, K;
   int lda, ldb, ldd;

@@ -172,6 +172,11 @@ __device__ __forceinline__ float2 load_16x2(const void* p) {   // two adjacent 1
   if constexpr (kBf16) return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p));
   else return __half22float2(*reinterpret_cast<const __half2*>(p));
 }
+template <bool kBf16>
+__device__ __forceinline__ float2 unpack_16x2(uint32_t w) {   // the two 16-bit values of a 32-bit word (low first) as floats
+  if constexpr (kBf16) return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w));
+  else return __half22float2(*reinterpret_cast<const __half2*>(&w));
+}
 __device__ __forceinline__ float gelu_tanh(float x) {
   // 0.5 x (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3)))
   const float k0 = 0.7978845608028654f, k1 = 0.044715f;
@@ -189,5 +194,7 @@ __device__ __forceinline__ float gelu_tanh_grad(float x) {
   float du = k0 * (1.f + 3.f * k1 * x2);
   return 0.5f * (1.f + t) + 0.5f * x * (1.f - t * t) * du;
 }
+// sigmoid of a SwiGLU gate: for a < -88 __expf(-a) overflows to inf and s = 0 exactly, so every SwiGLU product stays finite
+__device__ __forceinline__ float swiglu_sigmoid(float a) { return 1.f / (1.f + __expf(-a)); }
 
 }  // namespace pfx

@@ -48,8 +48,6 @@ def check_ffn_activation(m, d, compress) -> None:
         return
     if act != "swiglu":
         raise ValueError(f"Model.ffn_activation must be gelu or swiglu, got {act!r}")
-    if (m.get("moe_configs") or {}).get("expert_mode", False):
-        raise ValueError("ffn_activation: swiglu is not supported with moe_configs (the MoE experts keep the GELU FFN)")
     prune = compress.get("Prune") or {}
     if prune.get("enable", False):
         raise ValueError("Compress.Prune does not support ffn_activation: swiglu (FFN channel pruning would have to remove gate / up pairs)")
@@ -57,6 +55,22 @@ def check_ffn_activation(m, d, compress) -> None:
     if f and mp > 1 and f % mp:
         raise ValueError(f"ffn_hidden_size ({f}) must be divisible by mp_degree ({mp}) under ffn_activation: swiglu: "
                          "tensor parallelism shards whole gate / up pairs")
+
+
+def check_moe_configs(m, d) -> None:
+    """``Model.moe_configs``: every token goes to ``top_k`` distinct experts, so the experts of the whole job (``num_experts`` per rank, at
+    most one set per rank) must number at least ``top_k``; a gate cannot pick 2 of 1."""
+    mc = m.get("moe_configs") or {}
+    if not mc.get("expert_mode", False):
+        return
+    ranks = 1
+    for key in ("dp_degree", "mp_degree", "pp_degree", "cp_degree"):
+        ranks *= int(d.get(key, 1) or 1)
+    ranks *= int((d.get("sharding", {}) or {}).get("sharding_degree", 1) or 1)
+    n, k = int(mc.get("num_experts", 1)), int(mc.get("top_k", 2))
+    if k > n * ranks:
+        raise ValueError(f"Model.moe_configs.top_k ({k}) exceeds the number of experts ({n} per rank on {ranks} rank(s)): "
+                         "raise num_experts or lower top_k")
 
 
 def check_document_mask(m, d, data) -> None:
@@ -101,6 +115,7 @@ def check_config(cfg):
         raise ValueError("num_attention_heads must be divisible by mp_degree")
     check_kv_heads(m, d, cfg.get("Compress", {}) or {})
     check_ffn_activation(m, d, cfg.get("Compress", {}) or {})
+    check_moe_configs(m, d)
     check_document_mask(m, d, cfg.get("Data", {}) or {})
     logger.debug("config checks passed")
     return True

@@ -1,6 +1,7 @@
 """Throughput of the other BASELINE.json workloads (bench.py is reserved for the GPT-3 6.7B headline):
 
     moe    GPT-MoE 8 x 1.3B, expert parallel over the data-parallel ranks, gshard top-2, 2 experts / rank   (tokens/s)
+    moe-swiglu  the same model with SwiGLU experts (Model.ffn_activation: swiglu, F = 5632)               (tokens/s)
     vit    ViT-L/16 384^2 fine-tune, ZeRO stage 2 over all ranks, 32 images / GPU                            (images/s)
     ernie  ERNIE 10B-class encoder, mp x ZeRO stage 3                                                        (tokens/s)
     gpt-1.3b    GPT 1.3B (tanh-GELU FFN, 4h), data parallel, 8 x 1024 tokens / GPU                          (tokens/s)
@@ -31,7 +32,7 @@ CFG = os.path.join(ROOT, "paddlefleetx_b200", "configs")
 
 def parse():
     p = argparse.ArgumentParser()
-    p.add_argument("--workload", required=True, choices=["moe", "vit", "ernie", "gpt-1.3b", "gpt-swiglu", "gpt-1.3b-docs"])
+    p.add_argument("--workload", required=True, choices=["moe", "moe-swiglu", "vit", "ernie", "gpt-1.3b", "gpt-swiglu", "gpt-1.3b-docs"])
     p.add_argument("--gpus", type=int, default=1)
     p.add_argument("--steps", type=int, default=5)
     p.add_argument("--warmup", type=int, default=3)
@@ -95,11 +96,14 @@ def main():
             else:
                 pos = torch.arange(seq).unsqueeze(0).expand(local, seq).contiguous()
             return [t[:, :-1].contiguous(), pos, t[:, 1:].contiguous(), torch.ones(local, seq)]
-    elif a.workload == "moe":
+    elif a.workload in ("moe", "moe-swiglu"):
         local = a.local_batch or 8
+        swiglu = a.workload == "moe-swiglu"
         ov = common + [f"Global.local_batch_size={local}", f"Global.micro_batch_size={local}", f"Distributed.dp_degree={world}",
                        "Distributed.mp_degree=1", "Distributed.pp_degree=1", "Distributed.sharding.sharding_degree=1",
                        f"Model.moe_configs.fused_p2p={bool(a.p2p)}", "Model.use_recompute=False"]
+        if swiglu:
+            ov.append("Model.ffn_activation=swiglu")
         if a.layers:
             ov.append(f"Model.num_layers={a.layers}")
         cfg = C.get_config(os.path.join(CFG, "nlp/moe/pretrain_moe_1.3B_dp8.yaml"), ov, nranks=world)
@@ -107,7 +111,13 @@ def main():
         cfg.Data.Train["dataset"] = C.AttrDict(name="SyntheticGPTDataset", max_seq_len=seq, vocab_size=cfg.Model.vocab_size)
         cfg.Data.Train["loader"] = C.AttrDict(num_workers=0, collate_fn="gpt_collate_fn")
         unit, per_step = "tokens/s", local * seq * world
-        name = f"GPT-MoE {world}x1.3B (2 experts/rank, gshard top-2), expert parallel over dp{world}, {'peer-memory' if a.p2p else 'NCCL all-to-all'} dispatch"
+        if swiglu:
+            from paddlefleetx_b200.models.language_model.gpt.model import swiglu_ffn_size
+
+            experts = f"2 SwiGLU experts/rank, F = {cfg.Model.get('ffn_hidden_size') or swiglu_ffn_size(cfg.Model.hidden_size)}"
+        else:
+            experts = "2 experts/rank"
+        name = f"GPT-MoE {world}x1.3B ({experts}, gshard top-2), expert parallel over dp{world}, {'peer-memory' if a.p2p else 'NCCL all-to-all'} dispatch"
 
         def make_batch(g):
             t = torch.randint(0, cfg.Model.vocab_size, (local, seq + 1), generator=g)
