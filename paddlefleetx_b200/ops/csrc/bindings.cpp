@@ -488,6 +488,7 @@ std::vector<at::Tensor> topp_sampling(const at::Tensor& probs, const at::Tensor&
   PFX_CHECK_CUDA_CONTIG(probs);
   const c10::cuda::CUDAGuard guard(probs.device());
   const int64_t V = probs.size(-1), rows = probs.numel() / V;
+  TORCH_CHECK(top_ps.device() == probs.device(), "topp_sampling: top_ps must be on ", probs.device(), ", got ", top_ps.device());
   auto tp = top_ps.to(at::kFloat).contiguous();
   TORCH_CHECK(tp.numel() == rows, "top_ps must have one entry per row");
   auto out_p = at::empty({rows, 1}, probs.options().dtype(at::kFloat));
@@ -675,9 +676,21 @@ void adamw_symm_broadcast_(int64_t mc_params, const std::vector<int64_t>& peer_p
                                            dtype_code(grad), (int)lp_dtype, (int)rank, (int)pp.size(), (int)num_ctas, cur_stream()));
 }
 
+// The skinny GEMV reads x, w, ln_w and ln_b with 16-byte loads and every operand as x's dtype.  `op` names the binding in the messages.
+static void check_gemv_operands(const char* op, const at::Tensor& x, const at::Tensor& w, const c10::optional<at::Tensor>& bias) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && w.dim() == 2 && x.is_contiguous() && w.is_contiguous() && x.size(1) == w.size(1), op, ": x [M,K], w [N,K]");
+  TORCH_CHECK(w.device() == x.device(), op, ": w must be on ", x.device());
+  TORCH_CHECK(x.scalar_type() == w.scalar_type(), op, ": dtype mismatch");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0, op, ": x must be 16-byte aligned");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(w.data_ptr()) % 16 == 0, op, ": w must be 16-byte aligned");
+  if (bias.has_value() && bias->defined())
+    TORCH_CHECK(bias->device() == x.device() && bias->is_contiguous() && bias->scalar_type() == x.scalar_type() && bias->numel() == w.size(0), op,
+                ": bias must be a contiguous [", w.size(0), "] tensor of dtype ", x.scalar_type(), " on ", x.device(), ", got ", bias->scalar_type(), " ",
+                bias->sizes(), " on ", bias->device());
+}
+
 at::Tensor gemv_skinny(const at::Tensor& x, const at::Tensor& w, c10::optional<at::Tensor> bias) {
-  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && w.dim() == 2 && x.is_contiguous() && w.is_contiguous() && x.size(1) == w.size(1), "gemv_skinny: x [M,K], w [N,K]");
-  TORCH_CHECK(x.scalar_type() == w.scalar_type(), "gemv_skinny: dtype mismatch");
+  check_gemv_operands("gemv_skinny", x, w, bias);
   at::Tensor y = at::empty({x.size(0), w.size(0)}, x.options());
   const void* b = (bias.has_value() && bias->defined()) ? bias->data_ptr() : nullptr;
   PFX_CUDA_CHECK(pfx::gemv_skinny(x.data_ptr(), w.data_ptr(), b, y.data_ptr(), (int)x.size(0), (int)w.size(0), (int)x.size(1), dtype_code(x),
@@ -687,16 +700,23 @@ at::Tensor gemv_skinny(const at::Tensor& x, const at::Tensor& w, c10::optional<a
 
 at::Tensor gemv_fused(const at::Tensor& x, const at::Tensor& w, c10::optional<at::Tensor> bias, c10::optional<at::Tensor> ln_w,
                       c10::optional<at::Tensor> ln_b, double ln_eps, c10::optional<at::Tensor> residual, int64_t act) {
-  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && w.dim() == 2 && x.is_contiguous() && w.is_contiguous() && x.size(1) == w.size(1), "gemv_fused: x [M,K], w [N,K]");
-  TORCH_CHECK(x.scalar_type() == w.scalar_type(), "gemv_fused: dtype mismatch");
+  check_gemv_operands("gemv_fused", x, w, bias);
   TORCH_CHECK(act >= 0 && act <= 2, "gemv_fused: act must be 0 (none), 1 (GELU) or 2 (SwiGLU), got ", act);
   TORCH_CHECK(act != 2 || w.size(0) % 2 == 0, "gemv_fused: SwiGLU needs an even number of weight rows (gate, up pairs), got ", w.size(0));
   at::Tensor y = at::empty({x.size(0), act == 2 ? w.size(0) / 2 : w.size(0)}, x.options());
   auto ptr = [](const c10::optional<at::Tensor>& t) -> const void* { return (t.has_value() && t->defined()) ? t->data_ptr() : nullptr; };
   if (residual.has_value() && residual->defined())
-    TORCH_CHECK(residual->is_contiguous() && residual->numel() == y.numel() && residual->scalar_type() == x.scalar_type(), "gemv_fused: residual [M,N]");
-  if (ln_w.has_value() && ln_w->defined())
-    TORCH_CHECK(ln_w->numel() == x.size(1) && ln_b.has_value() && ln_b->numel() == x.size(1) && ln_w->scalar_type() == x.scalar_type(), "gemv_fused: ln params [K]");
+    TORCH_CHECK(residual->device() == x.device() && residual->is_contiguous() && residual->numel() == y.numel() && residual->scalar_type() == x.scalar_type(),
+                "gemv_fused: residual [M,N]");
+  TORCH_CHECK((ln_w.has_value() && ln_w->defined()) == (ln_b.has_value() && ln_b->defined()), "gemv_fused: ln_w and ln_b come together");
+  if (ln_w.has_value() && ln_w->defined()) {
+    for (const at::Tensor* t : {&*ln_w, &*ln_b}) {
+      TORCH_CHECK(t->device() == x.device() && t->is_contiguous() && t->numel() == x.size(1) && t->scalar_type() == x.scalar_type(),
+                  "gemv_fused: ln params must be contiguous [", x.size(1), "] tensors of dtype ", x.scalar_type(), " on ", x.device(), ", got ",
+                  t->scalar_type(), " ", t->sizes(), " on ", t->device());
+      TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, "gemv_fused: ln params must be 16-byte aligned");
+    }
+  }
   PFX_CUDA_CHECK(pfx::gemv_skinny(x.data_ptr(), w.data_ptr(), ptr(bias), y.data_ptr(), (int)x.size(0), (int)w.size(0), (int)x.size(1), dtype_code(x),
                                   at::cuda::getCurrentDeviceProperties()->multiProcessorCount, cur_stream(), ptr(ln_w), ptr(ln_b), (float)ln_eps,
                                   ptr(residual), (int)act));

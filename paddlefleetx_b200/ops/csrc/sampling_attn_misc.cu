@@ -6,7 +6,8 @@
 //   (2) otherwise a 4-pass radix *descent* on the float bit pattern with mass histograms: it finds the
 //       probability value t at which the descending cumulative mass crosses u — i.e. the token the sorted
 //       prefix-sum search would have returned — in 4 reads of an L2-resident row,
-//   (3) tie resolution in index order.
+//   (3) among the tokens of exactly that value, the one the sorted search reaches first (ties in index order), with no cap on
+//       the number of ties.
 // RNG is a stateless Philox counter (seed, offset+row): reproducible, no state tensor, graph-capturable.
 #include "pfx_common.cuh"
 #include "pfx_kernels.h"
@@ -25,7 +26,7 @@ topp_sampling_kernel(const T* __restrict__ probs, const float* __restrict__ top_
   __shared__ int s_idx[32];
   __shared__ uint32_t s_prefix;
   __shared__ float s_mass_above;
-  __shared__ int s_sel;
+  __shared__ int s_sel, s_rank;
   const int row = blockIdx.x;
   const T* pr = probs + (size_t)row * V;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -123,35 +124,64 @@ topp_sampling_kernel(const T* __restrict__ probs, const float* __restrict__ top_
   const uint32_t tkey = s_prefix;
   const float t = __uint_as_float(tkey);
 
-  // ---- (3) k-th (index order) among exact ties
-  int k = (t > 0.f) ? (int)floorf((u - s_mass_above) / t) : 0;
-  if (k < 0) k = 0;
-  if (k > 31) k = 31;
-  int last = -1;
-  for (int round = 0; round <= k; ++round) {
-    int best = 0x7fffffff;
-    for (int i = threadIdx.x; i < V; i += blockDim.x) {
-      if (i > last && __float_as_uint(to_f32<T>(pr[i])) == tkey) { best = i; break; }   // per-thread indices ascend
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
-    __syncthreads();
-    if (lane == 0) s_idx[w] = best;
-    __syncthreads();
-    if (w == 0) {
-      best = s_idx[lane];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
-      if (lane == 0) s_sel = best;
-    }
-    __syncthreads();
-    if (s_sel == 0x7fffffff) break;   // fewer ties than k: keep the previous one
-    last = s_sel;
+  // ---- (3) tie number j (in index order) among the tokens of value exactly t.  Warp w owns the contiguous span
+  // [w * span, (w + 1) * span) of the row and reads it 32 consecutive tokens at a time, so its reads stay coalesced and a ballot lists the
+  // ties of each step in index order.  One counting pass, an exclusive scan of the 32 warp counts, then the owning warp walks its span.
+  static_assert(kTopPThreads == 32 * 32, "the tie scan below is one warp wide: one count per warp");
+  const int span = ((V + 31) / 32 + 31) & ~31;
+  const int lo = min(V, w * span), hi = min(V, lo + span);
+  int cnt = 0;
+  for (int b = lo; b < hi; b += 32) {
+    const int i = b + lane;
+    cnt += __popc(__ballot_sync(0xffffffffu, i < hi && __float_as_uint(to_f32<T>(pr[i])) == tkey));
   }
-  if (threadIdx.x == 0) {
-    const int id = last < 0 ? imax : last;
-    out_prob[row] = to_f32<T>(pr[id]);
-    out_id[row] = id;
+  if (lane == 0) s_idx[w] = cnt;
+  __syncthreads();
+  if (w == 0) {
+    const int c = s_idx[lane];
+    int incl = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += v;
+    }
+    const int ties = __shfl_sync(0xffffffffu, incl, 31);
+    // the first tie whose cumulative mass reaches u: the smallest j with above + (j + 1) t >= u, evaluated in double (a product (j + 1) t
+    // of a 24-bit t is exact there) rather than by an approximate fp32 division; j is clamped to the last tie when rounding overshoots
+    const double need = (double)u - (double)s_mass_above;
+    int j = 0;
+    if (ties > 0 && t > 0.f && need > 0.0) {
+      const double q = ceil(need / (double)t) - 1.0;
+      j = q < 0.0 ? 0 : (q > (double)(ties - 1) ? ties - 1 : (int)q);
+      while (j > 0 && (double)j * t >= need) --j;
+      while (j < ties - 1 && (double)(j + 1) * t < need) ++j;
+    }
+    const int excl = incl - c;
+    const unsigned owner = __ballot_sync(0xffffffffu, c > 0 && j >= excl && j < incl);
+    if (lane == 0) s_sel = ties > 0 ? (int)__ffs(owner) - 1 : -1;
+    if (ties > 0 && lane == (int)__ffs(owner) - 1) s_rank = j - excl;
+  }
+  __syncthreads();
+  if (s_sel < 0) {                    // no token has value t (a row without positive mass): the arg-max
+    if (threadIdx.x == 0) { out_prob[row] = pmax; out_id[row] = imax; }
+    return;
+  }
+  if (w == s_sel) {
+    int r = s_rank;
+    for (int b = lo; b < hi; b += 32) {
+      const int i = b + lane;
+      const unsigned m = __ballot_sync(0xffffffffu, i < hi && __float_as_uint(to_f32<T>(pr[i])) == tkey);
+      const int n = __popc(m);
+      if (r < n) {
+        if (lane == 0) {
+          const int id = b + (int)__fns(m, 0, r + 1);
+          out_prob[row] = to_f32<T>(pr[id]);
+          out_id[row] = id;
+        }
+        break;
+      }
+      r -= n;
+    }
   }
 }
 

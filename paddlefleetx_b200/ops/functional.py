@@ -198,7 +198,7 @@ class _LinearFn(torch.autograd.Function):
 
 def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
     """weight is ``[out, in]``."""
-    if (x.is_cuda and x.dtype == weight.dtype and x.dtype in (torch.bfloat16, torch.float16) and weight.is_contiguous()
+    if (x.is_cuda and tensor_core_dtype(x, weight, bias) and weight.is_contiguous()
             and x.numel() // x.shape[-1] <= _GEMV_MAX_ROWS and x.shape[-1] % 8 == 0 and not (torch.is_grad_enabled() and (x.requires_grad or weight.requires_grad))
             and _native.available()):
         # token-by-token decoding: a weight stream, not a tensor-core problem (csrc/gemv_skinny.cu)

@@ -1,11 +1,12 @@
 """SwiGLU on the sm_90a kernels (needs an H100): ``bias_swiglu`` forward / backward and the SwiGLU decode GEMV against float64 within the
-bounds of ``swiglu_refs``, a SwiGLU GPT that trains with no library GEMM or activation kernel, and CUDA-graph decoding."""
+bounds of ``swiglu_refs`` and ``decode_refs``, a SwiGLU GPT that trains with no library GEMM or activation kernel, and CUDA-graph decoding."""
 import os
 
 import numpy as np
 import pytest
 import torch
 
+import decode_refs as D
 import kernel_refs as R
 import swiglu_refs as S
 from paddlefleetx_b200.ops import _native
@@ -95,29 +96,6 @@ def test_bias_swiglu_rejects_bad_shapes():
 
 
 # ---------------------------------------------------------------------------------------------------------------- decode GEMV
-def _gemv_ref(x, w, b, ln, res):
-    """float64 reference of the SwiGLU GEMV and its bound: the GEMV's fp32 dot products (within 2^-24 K of the sum of |terms|) and the LN
-    prologue's fp32 statistics enter the pre-activations; ``swiglu_bound`` covers the finish."""
-    xd, xmag = R._d(x), R._d(x).abs()
-    if ln is not None:
-        xd, mean, rstd = R.layer_norm(x, ln[0], ln[1], ln[2])
-        # fp32 statistics over K err by up to ~K 2^-24 relatively; (x - mean) rstd gamma + beta is bounded elementwise by this magnitude
-        xmag = (R._d(x).abs() + mean.abs()[:, None]) * rstd[:, None] * R._d(ln[0]).abs() + R._d(ln[1]).abs()
-    z = xd @ R._d(w).t() + (R._d(b) if b is not None else 0.0)
-    terms = xmag @ R._d(w).abs().t() + (R._d(b).abs() if b is not None else 0.0)
-    K = x.shape[-1]
-    dz = terms * R.FP32_U * (2 * K + 16)              # absolute error of each pre-activation before the finish
-    h = S.swiglu(z)
-    a, bb = z[:, 0::2], z[:, 1::2]
-    s = torch.sigmoid(a)
-    # a moves h by |d h / d a| = |b s (1 + a (1 - s))|, b by |a s|
-    E = S.swiglu_bound(z)["scale"] + (bb * s * (1 + a * (1 - s))).abs() * dz[:, 0::2] + (a * s).abs() * dz[:, 1::2]
-    if res is not None:
-        h = h + R._d(res)
-        E = E + R.FP32_U * h.abs()
-    return h, dict(scale=E, approx=1.0)
-
-
 @pytest.mark.parametrize("dtype", DTYPES)
 @pytest.mark.parametrize("rows", [1, 2, 3, 5, 8])
 @pytest.mark.parametrize("ln,res", [(False, False), (True, False), (True, True), (False, True)])
@@ -137,7 +115,7 @@ def test_gemv_swiglu_against_float64(dtype, rows, ln, res):
             _native.require().gemv_set_tuning(0, 0)
         torch.cuda.synchronize()
         assert y.shape == (rows, N // 2) and y.dtype == dtype
-        want, kw = _gemv_ref(x, w, b, lnp, r)
+        want, kw = D.gemv_ref(x, w, b, lnp, r, act="swiglu")
         _record("gemv swiglu", dtype, R.assert_close(y, want, dtype, **kw, what=f"gemv swiglu cols {cols} split {split}"))
 
 
