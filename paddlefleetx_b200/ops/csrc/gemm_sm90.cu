@@ -12,7 +12,7 @@
 //     accumulator fragment (registers -> swizzled smem -> TMA store).  One k-block of wgmma stays in flight while the next
 //     is issued; the producer runs ahead into the next tile during the epilogue.
 //   * tiles: 128 x 128 (288 threads) everywhere, and 128 x 256 (384 threads: warpgroup 2 is the producer and hands its registers to
-//     the consumers) for the plain 16-bit-output GEMM when the caller asks for it (GemmArgs::config == 1).  The wide tile fills the
+//     the consumers) for the plain 16-bit-output GEMM and the dGELU GEMM when the caller asks for it (GemmArgs::config == 1).  The wide tile fills the
 //     SM's registers and shared memory, so no side-stream kernel fits beside it: the training step asks for it in the backward only,
 //     where the single-GPU side stream carries nothing but the gradient-norm reduction (ops/functional.py).
 //
@@ -139,8 +139,11 @@ __device__ void ag_push_role(const GemmComm& c, int comm_cta, int num_comm_ctas,
 //           3 = bf16 scatter into the destination rank's staging buffer over NVLink (GEMM -> reduce-scatter),
 //           4 / 5 = the 16-bit TMA-store outputs of EPI_BIAS_SWIGLU_DUAL / EPI_DSWIGLU (kOutSwiGLU / kOutDSwiGLU; the launcher picks them from
 //           the epilogue, GemmArgs::out_mode stays 0).  They are modes of their own, not runtime epilogue branches, so the instantiations
-//           of modes 0-3 keep their registers: the 128 x 128 kernel sits at 162-168 of them.
-constexpr int kOutSwiGLU = 4, kOutDSwiGLU = 5;
+//           of modes 0-3 keep their registers: the 128 x 128 kernel sits at 158-159 of them.
+//           6 = the 16-bit TMA-store output of EPI_DGELU (kOutDGelu): the producer TMA-loads the saved pre-activation z into the
+//           epilogue staging buffers, each consumer thread multiplies its accumulators by gelu'(z) read from, and written back to, the
+//           same swizzled addresses, and the producer stores the buffer (see the producer for the order of its loads and stores).
+constexpr int kOutSwiGLU = 4, kOutDSwiGLU = 5, kOutDGelu = 6;
 
 template <int kBlockN, bool kAK, bool kBK, int kOutMode, bool kBf16>
 __global__ void __launch_bounds__(GemmSmem<kBlockN>::kThreads, 1)
@@ -152,8 +155,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
                   const uint16_t* __restrict__ aux, int ld_aux, const __grid_constant__ GemmGroup grp) {
   using S = GemmSmem<kBlockN>;
   constexpr int kStages = S::kStages;
+  constexpr int kChunks = kBlockN / kStoreCols;   // store boxes per tile
   static_assert(kStages >= 2, "pipeline needs at least two stages");
-  static_assert(!S::kWide || kOutMode == 0, "the wide tile serves the 16-bit TMA-store output only");
+  static_assert(!S::kWide || kOutMode == 0 || kOutMode == kOutDGelu, "the wide tile serves the 16-bit TMA-store outputs of EPI_NONE / EPI_BIAS / EPI_DGELU only");
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -162,6 +166,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   const uint32_t smem_bar = smem_epi + S::kNumEpiBufs * S::kEpiBytes;
   auto full_bar = [&](int s) { return smem_bar + 8u * s; };
   auto empty_bar = [&](int s) { return smem_bar + 8u * (kStages + s); };
+  // kOutDGelu, per staging buffer b: z has landed in it (aux_full), the consumers have written the products over it (epi_full)
+  auto aux_full_bar = [&](uint32_t b) { return smem_bar + 8u * (2 * kStages + b); };
+  auto epi_full_bar = [&](uint32_t b) { return smem_bar + 8u * (2 * kStages + 2 + b); };
 
   const uint32_t warp = warp_id();
   const uint32_t lane = lane_id();
@@ -194,6 +201,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     if (kOutMode == 0 || kOutMode >= kOutSwiGLU) tma_prefetch_desc(&tmap_d);
     if (kOutMode == 3) { for (int i = 0; i < comm.world; ++i) tma_prefetch_desc(&peer_maps.m[i]); }
     for (int s = 0; s < kStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kNumConsumerWarps); }
+    if constexpr (kOutMode == kOutDGelu) {
+      tma_prefetch_desc(&tmap_d2);
+      for (uint32_t b = 0; b < 2; ++b) { mbar_init(aux_full_bar(b), 1); mbar_init(epi_full_bar(b), kNumConsumerWarps * 32); }
+    }
     fence_barrier_init();
   }
   __syncthreads();
@@ -208,6 +219,54 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     }
     if (elect_one()) {
       int stage = 0; uint32_t phase = 0;
+      // kOutDGelu: the producer moves both z and the result through the two staging buffers, [128 rows x 64 columns] at a time.  Box q
+      // of this CTA's sequence (tile q / kChunks, chunk q % kChunks) uses buffer q & 1: z is loaded into it once the store of box q - 2
+      // has read it, and once the consumers have written the products over z the producer stores it.  Per tile it issues
+      //   ring k-blocks 0 .. kStages-1 | for each box q up to chunk 1 of this tile: store box q - 2, wait for it to be read, load z of q
+      //   | ring k-blocks kStages ..
+      // The first k-blocks only need the slots the previous tile's mainloop hands back, so they go out before the producer turns to that
+      // tile's epilogue, where the ring is full and the producer would otherwise idle.  There it stores the previous tile's boxes as the
+      // consumers finish them and refills each buffer right away: the wide tile's z chunks 2 and 3 while its chunks 1 and 2 are computed,
+      // this tile's chunks 0 and 1 to land under its mainloop.  The consumers never wait for a store.
+      // prev_tc / cur_tc: the tiles tile_seq - 2 and tile_seq - 1 as m_blk << 16 | n_blk (boxes never lie further back; one register
+      // each: the wide producer has 40, and what does not fit spills)
+      uint32_t tile_seq = 0, prev_tc = 0, cur_tc = 0;
+      auto box_xy = [&](uint32_t q, int& row, int& col) {
+        const uint32_t t = q / kChunks + 1 == tile_seq ? cur_tc : prev_tc;
+        row = (int)(t >> 16) * kBlockM;
+        col = (int)(t & 0xffffu) * kBlockN + (int)(q % kChunks) * kStoreCols;
+      };
+      auto store_box_q = [&](uint32_t q) {
+        const uint32_t b = q & 1u;
+        int row, col;
+        box_xy(q, row, col);
+        mbar_wait(epi_full_bar(b), (q >> 1) & 1u);
+        if (col < N) tma_store_2d(&tmap_d, smem_epi + b * S::kEpiBytes, col, row);
+        tma_store_commit();
+      };
+      auto advance_boxes = [&](uint32_t q0, uint32_t q_end) {   // load z of boxes q0 .. q_end - 1, storing box q - 2 first
+        for (uint32_t q = q0; q < q_end; ++q) {
+          const uint32_t b = q & 1u;
+          if (q >= 2) {
+            store_box_q(q - 2);
+            tma_store_wait_read<0>();
+          }
+          int row, col;
+          box_xy(q, row, col);
+          if (col < N) {
+            mbar_arrive_expect_tx(aux_full_bar(b), S::kEpiBytes);
+            tma_load_2d(&tmap_d2, aux_full_bar(b), smem_epi + b * S::kEpiBytes, col, row);
+          } else {
+            mbar_arrive(aux_full_bar(b));   // a box right of the tensor: nothing of it is stored
+          }
+        }
+      };
+      auto tile_boxes = [&](const TileCoord& tc) {
+        prev_tc = cur_tc; cur_tc = (uint32_t)tc.m_blk << 16 | (uint32_t)tc.n_blk;
+        ++tile_seq;
+        advance_boxes(tile_seq == 1 ? 0 : (tile_seq - 2) * kChunks + 2, (tile_seq - 1) * kChunks + 2);
+        if constexpr (S::kWide) tile_grid(opaque(M), opaque(N), opaque(K));   // formed anew rather than kept live (and spilled) across the boxes
+      };
       for (int tile = cta_id; tile < num_tiles; tile += num_ctas) {
         const TileCoord tc = tile_coord(tile, num_m_blocks, num_n_blocks, m_rotate);
         int m_idx = tc.m_blk * kBlockM;
@@ -224,6 +283,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           m_idx -= g * grp.m_per_group;
         }
         for (int kb = 0; kb < tile_k_blocks; ++kb) {
+          if constexpr (kOutMode == kOutDGelu) { if (kb == kStages) tile_boxes(tc); }
           mbar_wait(empty_bar(stage), phase ^ 1u);
           const uint32_t sa = smem_ab + stage * S::kStageBytes;
           const uint32_t sb = sa + S::kABytes;
@@ -261,6 +321,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           }
           if (++stage == kStages) { stage = 0; phase ^= 1u; }
         }
+        if constexpr (kOutMode == kOutDGelu) { if (tile_k_blocks <= kStages) tile_boxes(tc); }
+      }
+      if constexpr (kOutMode == kOutDGelu) {   // the last tile's remaining z chunks, then its stores
+        if (tile_seq > 0) {
+          advance_boxes((tile_seq - 1) * kChunks + 2, tile_seq * kChunks);
+          for (uint32_t q = tile_seq * kChunks - 2; q < tile_seq * kChunks; ++q) store_box_q(q);
+        }
+        tma_store_wait<0>();
       }
     }
   } else {
@@ -306,6 +374,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             asm volatile("prefetch.global.L2 [%0];" ::"l"(aux + (size_t)grow * ld_aux + 2 * col_tile + (lane & 3u) * 64u));
         }
       }
+      if constexpr (kOutMode == kOutDGelu && kChunks > 2) {
+        // z chunks 2.. reuse a staging buffer, so the producer loads them during the epilogue: pull them into L2 now, under the mainloop.
+        // Columns [128, 256) of the tile are two 128-byte lines per row; the 4 threads of a row pair take one line each.
+        static_assert(kChunks == 4, "chunks 2 and 3 are one 128-byte line each");
+        const int grow = row0 + (int)row_lo + 8 * (int)((lane >> 1) & 1u);
+        const int gcol = col_tile + 2 * kStoreCols + (int)(lane & 1u) * kStoreCols;
+        if (grow < M && gcol < N) asm volatile("prefetch.global.L2 [%0];" ::"l"(aux + (size_t)grow * ld_aux + gcol));
+      }
       int prev_stage = -1;
       for (int kb = 0; kb < tile_k_blocks; ++kb) {
         mbar_wait(full_bar(stage), phase);
@@ -342,7 +418,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 #pragma unroll
           for (int i = 0; i < 32; ++i) v[i] = empty_k ? 0.f : acc[c * 32 + i];
         }
-        if (kOutMode == kOutSwiGLU || (kOutMode != kOutDSwiGLU && (epilogue == EPI_BIAS || epilogue == EPI_BIAS_GELU || epilogue == EPI_BIAS_GELU_DUAL))) {
+        if (kOutMode == kOutSwiGLU || (kOutMode < kOutSwiGLU && (epilogue == EPI_BIAS || epilogue == EPI_BIAS_GELU || epilogue == EPI_BIAS_GELU_DUAL))) {
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             if (cb + 8 * j < N) {   // N % 8 == 0 is required by the host wrapper
@@ -351,25 +427,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             }
           }
         }
-        if (!S::kWide && kOutMode < kOutSwiGLU && (epilogue == EPI_BIAS_GELU || epilogue == EPI_GELU)) {   // the wide tile serves EPI_NONE / EPI_BIAS / EPI_DGELU
+        if (!S::kWide && kOutMode < kOutSwiGLU && (epilogue == EPI_BIAS_GELU || epilogue == EPI_GELU)) {   // the wide tile serves EPI_NONE / EPI_BIAS
 #pragma unroll
           for (int i = 0; i < 32; ++i) v[i] = gelu_tanh(v[i]);
-        }
-        if (kOutMode < kOutSwiGLU && epilogue == EPI_DGELU) {      // acc * gelu'(saved pre-activation)
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            const int grow_aux = row0 + (int)row_lo + 8 * hh;
-            if (grow_aux < M) {
-              const uint16_t* ap = aux + (size_t)grow_aux * ld_aux + cb;
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                if (cb + 8 * j < N) {
-                  const float2 f = load_16x2<kBf16>(ap + 8 * j);
-                  v[4 * j + 2 * hh] *= gelu_tanh_grad(f.x); v[4 * j + 2 * hh + 1] *= gelu_tanh_grad(f.y);
-                }
-              }
-            }
-          }
         }
         if constexpr (kOutMode != 1 && kOutMode != 2) {
           // fill(box) writes one store box into the next staging buffer, which is then TMA-stored at column x of the tile's rows; called
@@ -455,6 +515,38 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
                 }
               });
             }
+          } else if constexpr (kOutMode == kOutDGelu) {
+            // v * gelu'(z): the staging buffer holds z's box, swizzled like the output, so every thread finds its own elements of z where
+            // fill_v would write them and overwrites them with the product; the producer stores the buffer.  Past the right edge of the
+            // tensor the buffer holds zeros or stale data; those columns are not stored.
+            const uint32_t buf = store_iter & 1u;
+            const uint32_t box = smem_epi + buf * S::kEpiBytes;
+            mbar_wait(aux_full_bar(buf), (store_iter >> 1) & 1u);
+            uint32_t addr[2][8], zw[2][8];
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              const uint32_t r = row_lo + 8u * hh;
+              uint32_t sbase = box + r * 128u + col_in8 * 2u;
+              uint32_t r_sw = r & 7u;
+              if constexpr (S::kWide) { sbase = opaque(sbase); r_sw = opaque(r_sw); }   // as in fill_v
+#pragma unroll
+              for (int j = 0; j < 8; ++j) {
+                addr[hh][j] = sbase + (((uint32_t)j ^ r_sw) << 4);
+                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(zw[hh][j]) : "r"(addr[hh][j]) : "memory");
+              }
+            }
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+              for (int j = 0; j < 8; ++j) {
+                const float2 z = unpack_16x2<kBf16>(zw[hh][j]);
+                const uint32_t p = pack_16x2<kBf16>(v[4 * j + 2 * hh] * gelu_tanh_grad(z.x), v[4 * j + 2 * hh + 1] * gelu_tanh_grad(z.y));
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr[hh][j]), "r"(p) : "memory");
+              }
+            }
+            fence_proxy_async_smem();   // the products, written through the generic proxy, are read by the producer's TMA store
+            mbar_arrive(epi_full_bar(buf));
+            ++store_iter;
           } else {
             store_box(&tmap_d, col0, fill_v);
             if constexpr (kOutMode == kOutSwiGLU) {
@@ -502,7 +594,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         }
       }
     }
-    if (kOutMode != 1 && kOutMode != 2 && is_store_thread) tma_store_wait<0>();
+    if (kOutMode != 1 && kOutMode != 2 && kOutMode != kOutDGelu && is_store_thread) tma_store_wait<0>();
   }
 }
 
@@ -666,8 +758,13 @@ static cudaError_t launch_cfg(const GemmArgs& g, cudaStream_t stream) {
     if (g.d2 == nullptr || g.bias == nullptr || g.N % 16) return gemm_reject(g, kBlockN, __LINE__);
     ok &= make_tmap_2d_plain(&td2, g.d2, dt, g.N / 2, g.M, (uint64_t)g.N, kStoreCols / 2, kBlockM);
   }
-  if ((g.epilogue == EPI_DGELU || kOutMode == kOutDSwiGLU) && (g.aux == nullptr || g.ld_aux % 8 || (reinterpret_cast<uintptr_t>(g.aux) & 15)))
+  if ((kOutMode == kOutDGelu || kOutMode == kOutDSwiGLU) && (g.aux == nullptr || g.ld_aux % 8 || (reinterpret_cast<uintptr_t>(g.aux) & 15)))
     return gemm_reject(g, kBlockN, __LINE__);
+  if (kOutMode == kOutDGelu) {   // z [M, N], loaded box by box into the staging buffers: the same geometry as the output's
+    if ((g.M + kBlockM - 1) / kBlockM > 0xffff || (g.N + kBlockN - 1) / kBlockN > 0xffff)   // the producer keeps 16-bit tile coordinates
+      return gemm_reject(g, kBlockN, __LINE__);
+    ok &= make_tmap_2d(&td2, g.aux, 2, dt, g.N, g.M, (uint64_t)g.ld_aux * 2, kStoreCols, kBlockM);
+  }
   PeerMaps pm;
   for (int i = 0; i < 8; ++i) pm.m[i] = ta;
   if (kOutMode == 3) {
@@ -740,12 +837,19 @@ cudaError_t gemm_wgmma(const GemmArgs& g, cudaStream_t stream) {
     if (g.config != 0 || g.out_mode != 0 || g.group.mode != 1 || !g.a_kmajor || g.b_kmajor != fwd) return gemm_reject(g, 128, __LINE__);
     return fwd ? launch_cfg<128, true, true, kOutSwiGLU>(g, stream) : launch_cfg<128, true, false, kOutDSwiGLU>(g, stream);
   }
-  // The wide tile is compiled for the plain GEMM with a 16-bit output and the epilogues of the backward pass; any other request runs
-  // 128 x 128 and gives the same result.
+  // The dGELU epilogue serves the FFN2 dgrad, dense (gemm_dgelu) and grouped (the GELU experts): A K-major, B MN-major, 16-bit output.
+  if (g.epilogue == EPI_DGELU) {
+    if (g.out_mode != 0 || !g.a_kmajor || g.b_kmajor || g.group.mode == 2 || g.comm.rows_per_rank > 0 || g.comm.ag_world > 1)
+      return gemm_reject(g, 128, __LINE__);
+    return g.config == 1 && g.group.mode == 0 ? launch_cfg<kWideN, true, false, kOutDGelu>(g, stream)
+                                              : launch_cfg<128, true, false, kOutDGelu>(g, stream);
+  }
+  // The wide tile is compiled for the plain GEMM with a 16-bit output and the bias-free / bias epilogues of the backward pass; any other
+  // request runs 128 x 128 and gives the same result.
   const bool wide = g.config == 1 && g.out_mode == 0 && g.group.mode == 0 && g.comm.rows_per_rank == 0 && g.comm.ag_world <= 1 &&
-                    (g.epilogue == EPI_NONE || g.epilogue == EPI_BIAS || g.epilogue == EPI_DGELU);
+                    (g.epilogue == EPI_NONE || g.epilogue == EPI_BIAS);
   if (wide) return launch_major<kWideN, 0>(g, stream);
-  return launch_out<128>(g, stream);   // 128 x 128 tiles: 64 accumulator registers per consumer thread (162-168 registers in all; the eight out-mode-1 variants spill 44 bytes)
+  return launch_out<128>(g, stream);   // 128 x 128 tiles: 64 accumulator registers per consumer thread (158-159 registers in all, no spills)
 }
 
 }  // namespace pfx
